@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - the driver's benchmark contract for the jolt_b200 hot path.
+"""bench.py - the benchmark of the jolt_b200 hot path.
 
 Workload (BASELINE.json configs[1]): a complete degree-2 product sumcheck over m = 2 dense
 BN254-Fr tables of 2^22 entries per GPU - round 0 eval sweep, then 21 fused bind+eval passes and
@@ -17,6 +17,10 @@ e2e     : the same through the reference-facing call with HOST (pinned) tables: 
           cores) on the same workload - the reference itself is Rust and cannot be built here.
 N > 1   : weak scaling - each rank owns a contiguous 2^22 block of a global 2^(22+log2 N) polynomial
           (LowToHigh binding keeps pairs local), one NCCL all-reduce of the round sums per round.
+--dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step returned (the proof and the final
+          evaluations) as DIR/<name>.npy. Every 256-bit value is stored as its eight little-endian 32-bit words in
+          float64 (exact), so two builds can be compared output for output; the inputs are seeded, hence identical
+          from run to run with the same arguments.
 """
 from __future__ import annotations
 
@@ -52,6 +56,8 @@ def parse():
     ap.add_argument("--no-msm", action="store_true", help="skip the secondary G1 MSM measurement")
     ap.add_argument("--msm-log-n", type=int, default=20)
     ap.add_argument("--no-kernels", action="store_true", help="skip the per-kernel roofline section (bind, eq, MSM 2^20/2^24, HyperKZG, split-eq)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (256-bit values as 8 x u32 words, float64)")
     return ap.parse_args()
 
 
@@ -69,6 +75,17 @@ def all_ops(log_n: int, m: int) -> int:
     return total
 
 
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """arrays of u64 Montgomery limbs (..., 4) -> out_dir/<name>.npy as (..., 8) float64: the little-endian u32 words,
+    every one exactly representable, so equal files mean bit-identical field elements."""
+    import numpy as np
+    d = pathlib.Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype="<u8")
+        np.save(d / f"{name}.npy", a.view("<u4").reshape(a.shape[:-1] + (8,)).astype(np.float64))
+
+
 def config(args, world):
     return {
         "workload": f"product sumcheck, m={args.m} tables x 2^{args.log_n} BN254 Fr per GPU, degree {args.m}, "
@@ -76,15 +93,15 @@ def config(args, world):
         "log_n_per_gpu": args.log_n, "m": args.m, "order": args.order,
         "global_log_n": args.log_n + (world.bit_length() - 1),
         "field_ops_counted": "3 per bound output element (1 mul + 1 sub + 1 add), SURVEY 8d",
-        "l2": "a fresh input copy per step; per-step inputs (m x 2^n x 32 B) exceed the 126 MB L2",
+        "l2": "a fresh input copy per step; per-step inputs (m x 2^n x 32 B) exceed the 50 MB L2 of an H100",
         "parallelism": f"index-sharded x{world}" if world > 1 else "single GPU",
     }
 
 
 # ---------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock + throttle reasons sampled DURING the timed region (NVML, ~2 ms period; the
-    nvidia-smi loop of B200_PROFILING.md is too coarse for a timed region of tens of ms)."""
+    """SM clock + throttle reasons sampled DURING the timed region (NVML, ~2 ms period; an
+    nvidia-smi polling loop is too coarse for a timed region of tens of ms)."""
 
     def __init__(self, index: int):
         self.samples, self.reasons, self.smax, self._stop = [], set(), None, False
@@ -320,10 +337,11 @@ def kernels_section(sess, peak_hbm: float, with_cpu: bool):
         return t
 
     # the integer ceiling everything multiplier-bound is scored against
+    sm_count = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
     g_mul = {}
     for name, field, variant in (("fr_full", 0, 0), ("fr_challenge125", 0, 1), ("fq_full", 1, 0)):
         v = ctypes.c_double()
-        sess.check(sess.lib.jb_diag_mul_throughput(sess.h, field, variant, 2000, 148 * 8, ctypes.byref(v)))
+        sess.check(sess.lib.jb_diag_mul_throughput(sess.h, field, variant, 2000, sm_count * 8, ctypes.byref(v)))
         g_mul[name] = v.value
     out["montgomery_products_per_s"] = {k: v * 1e9 for k, v in g_mul.items()}
 
@@ -561,6 +579,10 @@ def run_ours(args):
     launches = sess.launch_count - launches0
     timed = sess.timing_collect()
     sess.timing_enable(False)
+    if args.dump_outputs and rank == 0:
+        ch, fin, mc, rp = res
+        dump_outputs(args.dump_outputs, {"challenges": ch, "final_claim": fin, "member_claims": mc,
+                                         "round_polys": rp, "final_evals": fe})
     if dist:
         tmax = torch.tensor([dev_ms], device="cuda")
         dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
@@ -621,7 +643,7 @@ def run_ours(args):
         peaks = json.load(open(ROOT / "MEASURED_PEAKS.json"))
     except Exception:
         pass
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", 3350.0)  # else the H100 SXM data-sheet HBM3 bandwidth
     big = [t for t in timed if t["kind"] == "fused_bind_eval" and t["items"] == n // 4]
     roof = None
     if big:
@@ -630,16 +652,8 @@ def run_ours(args):
         ach = alg_bytes / (avg_ms * 1e-3) / 1e9
         roof = {"bound": "hbm", "kernel": f"fused_round_kernel<M={m},{args.order},BIND,HI4> (round 1: 2^{args.log_n} -> 2^{args.log_n - 1})",
                 "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "fallback 6650 GB/s",
-                "algorithmic_bytes_per_launch": alg_bytes, "avg_launch_ms": avg_ms, "launches_timed": len(big),
-                "traffic": None}
-        try:  # dram__bytes_read.sum + dram__bytes_write.sum of this kernel from the committed ncu --set full capture
-            tr = json.load(open(ROOT / "profiles" / "r01b_traffic.json"))
-            if args.log_n == 22 and m == 2 and args.order == "l2h":
-                roof["traffic"] = tr["fused_round_kernel m=2 l2h 2^22"]["traffic"]
-                roof["traffic_source"] = tr["source"]
-        except Exception:
-            pass
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s",
+                "algorithmic_bytes_per_launch": alg_bytes, "avg_launch_ms": avg_ms, "launches_timed": len(big)}
         kernel_ms = sum(t["ms"] for t in timed) / K
         roof["timed_kernels_share_of_step"] = kernel_ms / ms_per_step
         # every timed streaming pass of a step (CUDA events on the launching stream, averaged over the K steps):

@@ -1,4 +1,4 @@
-/* jolt_b200.h - C ABI of the B200 (sm_100a) backend for the a16z/jolt prover hot path.
+/* jolt_b200.h - C ABI of the H100 (sm_90a) backend for the a16z/jolt prover hot path.
  *
  * The reference (a16z/jolt @ ff9f8c13) has no FFI today: its compute seam is a set of Rust
  * traits. Each entry point below names the reference interface it replaces (file:line under

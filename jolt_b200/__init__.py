@@ -1,4 +1,4 @@
-"""jolt_b200 - B200 (sm_100a) backend for the a16z/jolt prover hot path.
+"""jolt_b200 - H100 (sm_90a) backend for the a16z/jolt prover hot path.
 
 Python surface = thin ctypes bindings over the C ABI (include/jolt_b200.h) that mirror the
 reference's Rust types for this path:

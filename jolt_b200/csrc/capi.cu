@@ -1,4 +1,4 @@
-// C ABI of the B200 backend (see include/jolt_b200.h for the per-function reference citations).
+// C ABI of the H100 backend (see include/jolt_b200.h for the per-function reference citations).
 // The context mirrors ProofSession (crates/jolt-kernels/src/backend.rs:283-286): it owns the
 // stream, the stream-ordered device pool, and the small reduction / staging buffers.
 // This unit: library / context, tables, bind, eq expansion, element-wise harness, diagnostics.
@@ -111,8 +111,7 @@ int jbi::eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* sc
     if (st == JB_OK) st = c->dev_alloc((void**)&d_low8, 256 * 32);
     if (st == JB_OK) st = eq_build(c, r, hi_vars, scale, d_prefix);
     // layout (JB_EQ_LAYOUT: 0 (default) = the 3 register variables FIRST in the block, a warp's store covers 1 KiB;
-    // 1 = LAST: 8 consecutive outputs per thread. ncu A/B at 2^26 (profiles/r02_eq_store_ab.md): both write 2.0 x the
-    // table to DRAM whatever the store flavour, layout 0 is ~7 % faster)
+    // 1 = LAST: 8 consecutive outputs per thread; both write the same DRAM bytes whatever the store flavour)
     const bool low3 = c->eq_layout != 0;
     if (st == JB_OK) st = eq_build(c, r + 4 * (hi_vars + (low3 ? 0 : 3)), 8, nullptr, d_low8);
     if (st == JB_OK) {
@@ -149,7 +148,7 @@ int jbi::eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* sc
 // ------------------------------------------------------------------------------------------
 extern "C" {
 
-const char* jb_version(void) { return "jolt_b200 0.1 (sm_100a)"; }
+const char* jb_version(void) { return "jolt_b200 0.1 (sm_90a)"; }
 
 const char* jb_status_str(int status) {
     switch (status) {

@@ -68,7 +68,7 @@ struct jb_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool owns_stream = false;
-    int sm_count = 148;
+    int sm_count = 132;
     std::mutex mu;
     std::unordered_map<uint64_t, Table> tables;
     std::unordered_map<uint64_t, Srs> srs;

@@ -1,4 +1,4 @@
-// BN254 Fr / Fq Montgomery arithmetic for sm_100a, one element per thread, 8 x u32 limbs in
+// BN254 Fr / Fq Montgomery arithmetic for sm_90a, one element per thread, 8 x u32 limbs in
 // registers (memory layout = the reference's 4 x u64 little-endian Montgomery limbs,
 // crates/jolt-field/src/bn254/mod.rs:33-42; R = 2^256).
 //
@@ -517,17 +517,18 @@ __device__ __forceinline__ Fp<PR> reduce_wide17(const uint32_t* acc, int stride)
 using Fr = Fp<FrParams>;
 using Fq = Fp<FqParams>;
 
-// ---- 256-bit global memory access (one element = 32 B, naturally aligned) ----------------------
-// sm_100 has 256-bit LDG/STG (ld.global.v8.u32); one request per element, a warp covers 1 KiB
-// contiguous -> fully coalesced 32 B sectors.
+// ---- global memory access of one element (32 B, naturally aligned) ---------------------------
+// sm_90's widest LDG/STG is 128 bits: an element is two 16 B requests to the same 32 B sector, so a warp
+// still covers 1 KiB contiguous -> fully coalesced 32 B sectors. Only the read-only load is inline PTX (for
+// its L1::no_allocate hint); the others are plain vector accesses the compiler may schedule freely.
 template <class F>
 __device__ __forceinline__ F ld_elem(const uint64_t* base, size_t idx) {
     F r;
     const uint32_t* p = reinterpret_cast<const uint32_t*>(base) + idx * 8;
-    asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]),
-                   "=r"(r.v[6]), "=r"(r.v[7])
-                 : "l"(p));
+    asm("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+        : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]) : "l"(p));
+    asm("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+        : "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7]) : "l"(p + 4));
     return r;
 }
 
@@ -537,33 +538,34 @@ __device__ __forceinline__ void prefetch_l2(const uint64_t* base, size_t idx) {
     asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const uint32_t*>(base) + idx * 8));
 }
 
+template <class F>
+__device__ __forceinline__ F elem_from(const uint4& a, const uint4& b) {
+    F r;
+    r.v[0] = a.x, r.v[1] = a.y, r.v[2] = a.z, r.v[3] = a.w;
+    r.v[4] = b.x, r.v[5] = b.y, r.v[6] = b.z, r.v[7] = b.w;
+    return r;
+}
+
 // coherent variant for buffers written earlier in the same kernel / aliased in-place updates
 template <class F>
 __device__ __forceinline__ F ld_elem_rw(const uint64_t* base, size_t idx) {
-    F r;
-    const uint32_t* p = reinterpret_cast<const uint32_t*>(base) + idx * 8;
-    asm volatile("ld.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]),
-                   "=r"(r.v[6]), "=r"(r.v[7])
-                 : "l"(p));
-    return r;
+    const uint4* p = reinterpret_cast<const uint4*>(base) + idx * 2;
+    return elem_from<F>(p[0], p[1]);
 }
 
 template <class F>
 __device__ __forceinline__ void st_elem(uint64_t* base, size_t idx, const F& x) {
-    uint32_t* p = reinterpret_cast<uint32_t*>(base) + idx * 8;
-    asm volatile("st.global.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(x.v[0]), "r"(x.v[1]),
-                 "r"(x.v[2]), "r"(x.v[3]), "r"(x.v[4]), "r"(x.v[5]), "r"(x.v[6]), "r"(x.v[7])
-                 : "memory");
+    uint4* p = reinterpret_cast<uint4*>(base) + idx * 2;
+    p[0] = make_uint4(x.v[0], x.v[1], x.v[2], x.v[3]);
+    p[1] = make_uint4(x.v[4], x.v[5], x.v[6], x.v[7]);
 }
 
 // Streaming store (evict-first): for tables that are written once and not read again by the same kernel.
 template <class F>
 __device__ __forceinline__ void st_elem_cs(uint64_t* base, size_t idx, const F& x) {
-    uint32_t* p = reinterpret_cast<uint32_t*>(base) + idx * 8;
-    asm volatile("st.global.cs.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(x.v[0]), "r"(x.v[1]),
-                 "r"(x.v[2]), "r"(x.v[3]), "r"(x.v[4]), "r"(x.v[5]), "r"(x.v[6]), "r"(x.v[7])
-                 : "memory");
+    uint4* p = reinterpret_cast<uint4*>(base) + idx * 2;
+    __stcs(p, make_uint4(x.v[0], x.v[1], x.v[2], x.v[3]));
+    __stcs(p + 1, make_uint4(x.v[4], x.v[5], x.v[6], x.v[7]));
 }
 
 }  // namespace jb

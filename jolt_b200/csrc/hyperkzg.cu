@@ -328,7 +328,7 @@ int jb_hyperkzg_open(jb_ctx* c, jb_srs srs, jb_table evals, const uint64_t* poin
     {
         // The polynomials of <= 2^15 entries (the last min(ell - 1, 15) of them) are packed back to back with halving
         // lengths: one row-batched pass of the MSM pipeline commits them all (msm_halving_rows_device); 15 separate
-        // MSMs of that size are ~0.8 ms of launch latency each. The longer ones go one by one.
+        // MSMs of that size are latency-bound, one launch sequence each. The longer ones go one by one.
         const int h = ell >= 3 ? (int)(ell < 16 ? ell : 16) : 0;  // tail = the polynomials of lengths 2^(h-1) .. 2
         size_t off = 0, len = n / 2;
         size_t i = 1;

@@ -1,4 +1,4 @@
-// BN254 G1 multi-scalar multiplication (Pippenger bucket method) for sm_100a.
+// BN254 G1 multi-scalar multiplication (Pippenger bucket method) for sm_90a.
 // Replaces JoltGroup::msm (crates/jolt-crypto/src/ec/group.rs:70, impl ec/bn254/mod.rs:195-212 ->
 // ark_ec::VariableBaseMSM::msm_bigint) and therefore kzg_commit (crates/jolt-hyperkzg/src/kzg.rs:15-27).
 // The result is defined by value: sum_i [s_i] P_i with s_i the canonical integer of the scalar
@@ -34,8 +34,7 @@ namespace {
 
 // buckets per reduction segment: one thread walks a segment (2 general additions per bucket) and then multiplies the
 // segment's plain sum by its first bucket number (double-and-add, ~330 products): the multiplication is per SEGMENT, so
-// short segments cost work (measured at 2^20 / 2^24 terms, precomputed SRS: 8 buckets 0.88 / 3.76 ms, 16 buckets
-// 0.55 / 2.38 ms). JB_MSM_SEG overrides (A/B).
+// short segments cost work. JB_MSM_SEG overrides (A/B).
 int msm_seg_size(int buckets) {
     static const int env = [] {
         const char* e = getenv("JB_MSM_SEG");
@@ -43,7 +42,7 @@ int msm_seg_size(int buckets) {
         return x >= 2 && x <= 256 ? x : 0;
     }();
     if (env) return env;
-    return buckets >= (1 << 21) ? 64 : 16;  // 2^24 terms (2^21 buckets): 16 / 32 / 64 = 40.6 / 40.0 / 39.7 ms per MSM; 2^20 terms: 3.17 / 3.26 / 3.61
+    return buckets >= (1 << 21) ? 64 : 16;  // per-segment work shrinks with fewer, longer segments once buckets are many
 }
 
 struct MsmPlan {
@@ -394,7 +393,7 @@ __global__ void __launch_bounds__(256) msm_scatter_kernel(const uint32_t* digits
                                                           unsigned range_shift) {
     // mode 0: every window in this thread. The positions are random within the destination, and a random 4-byte
     // store dirties a 32-byte sector: once the destination (4 B x windows x terms) outgrows the L2, the scatter runs at
-    // the DRAM's sector rate (6.6 ms for 2^24 terms). So big MSMs order the work in TIME by destination region, one
+    // the DRAM's sector rate. So big MSMs order the work in TIME by destination region, one
     // grid row (blockIdx.y) per region, so that the region being filled stays in the L2 until its sectors are complete:
     // mode 1 (one bucket set per window): region = window; mode 2 (one shared bucket set): region = a bucket range
     // (slot >> range_shift); every row re-reads the digits (coalesced, cheap) and keeps its own entries.
@@ -876,10 +875,8 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
     const size_t max_tasks = nb + ((size_t)p.W * n) / MSM_CHUNK + 1;
     // Batched-affine levels (msm_affine.cuh): field scalars only (uniform digits: a bucket holds ~entries / nb points)
     // and only while a bucket still has several points per level. OFF by default: built, exact (tests force it at 2^13
-    // terms, exceptional pairs included) and measured SLOWER than the XYZZ accumulation it replaces - 2^24 terms,
-    // precomputed SRS: 30.6 ms of XYZZ accumulation (0.99 of the 10-products-per-addition ceiling once the tasks are
-    // walked in length order) against 35.2 / 36.2 / 38.2 ms with 2 / 3 / 4 affine levels in front of it; the level
-    // kernel reaches ~5.4 G additions/s = half of ITS ceiling (one thread's inversion idles its block, and the
+    // terms, exceptional pairs included) and measured SLOWER than the XYZZ accumulation it replaces; the level
+    // kernel stays far below ITS ceiling (one thread's inversion idles its block, and the
     // load - multiply - store chains of a thread expose the memory latency that the XYZZ walk hides behind 10 products).
     // JB_MSM_BA = levels switches it on, JB_MSM_BA_MIN_LOG = log2 of the smallest windows x terms product that takes
     // the path (tests lower it).
@@ -948,7 +945,7 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
                     regions = p.W;
                 } else if (p.c - 1 >= 6) {
                     mode = 2;
-                    int rl = 2;  // log2(regions); measured at 2^24 terms, 12 windows: 1 / 2 / 4 / 8 / 16 regions = 41.7 / 40.5 / 39.2 / 40.6 / 44.8 ms per MSM
+                    int rl = 2;  // log2(regions): more rows cost more digit re-reads than their L2 hits save
                     if (const char* e = getenv("JB_MSM_SCATTER_REGIONS_LOG")) rl = atoi(e);
                     if (rl < 0) rl = 0;
                     if (rl > 6) rl = 6;
@@ -1079,7 +1076,7 @@ void identity_xyz(uint64_t out[12]);
 
 // msm_binary on the device: `d_flags` = n bytes (0 / 1) already resident. Returns the Jacobian sum of the selected bases.
 int msm_binary_device(jb_ctx* c, const Srs& srs, size_t offset, const uint8_t* d_flags, size_t n, uint64_t out_xyz[12]) {
-    const unsigned blocks = 148 * 8;  // 1184 blocks x 128 threads: every thread owns ~n / 2^17 groups
+    const unsigned blocks = (unsigned)c->sm_count * 8;  // 8 blocks x 128 threads per SM (1056 on H100)
     const size_t T = (size_t)blocks * 128;
     uint64_t *partial = nullptr, *tree_a = nullptr, *tree_b = nullptr, *d_out = nullptr;
     int st = c->dev_alloc((void**)&partial, T * 128);
@@ -1322,7 +1319,7 @@ int jb_msm_g1_small(jb_ctx* c, jb_srs h, size_t offset, const void* scalars, siz
         st = c->dev_alloc((void**)&d_max, 4);
         if (st == JB_OK) st = c->check(cudaMemsetAsync(d_max, 0, 4, c->stream), "msm max memset");
         if (st == JB_OK) {
-            u8_max_kernel<<<148 * 4, 256, 0, c->stream>>>((const uint8_t*)d_s, n, d_max);
+            u8_max_kernel<<<(unsigned)c->sm_count * 4, 256, 0, c->stream>>>((const uint8_t*)d_s, n, d_max);
             c->launches++;
             st = c->check(cudaMemcpyAsync(c->h_small, d_max, 4, cudaMemcpyDeviceToHost, c->stream), "msm max D2H");
         }

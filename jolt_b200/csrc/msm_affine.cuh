@@ -21,7 +21,7 @@
 //            dependency chains per thread), parking the running prefixes in global scratch (32 B per pair, streaming);
 //   scan     prefix and suffix products of the 256 thread totals (shared memory), one Fermat inversion of the block total;
 //   phase 2  walking backwards, each thread peels 1 / d off its chains and finishes the additions.
-// The inversion is a serial chain of ~380 products on one thread (~0.2 ms); kp is chosen so that a block holds several
+// The inversion is a serial chain of ~380 products on one thread; kp is chosen so that a block holds several
 // times that much work and two resident blocks per SM cover each other's inversion.
 #pragma once
 #include "ec.cuh"

@@ -1,11 +1,11 @@
-// Device kernels for the sumcheck hot path over BN254 Fr (sm_100a):
+// Device kernels for the sumcheck hot path over BN254 Fr (sm_90a):
 //   * bind            - Polynomial::bind_with_order, crates/jolt-poly/src/dense.rs:180-263
 //                       (legacy DensePolynomial::bind, jolt-prover-legacy/src/poly/dense_mlpoly.rs:71-221)
 //   * fused bind+eval - the fused ProveRounds contract, crates/jolt-sumcheck/src/prover.rs:45-72,
 //                       restating NaiveSumcheckProver::prove_round (jolt-kernels/src/reference/naive.rs:241-310)
 //                       for Expr = product of m dense tables, degree m
 //   * eq expansion    - EqPolynomial::evals, crates/jolt-poly/src/eq.rs:221-231, 299-315 (r[0] <-> MSB)
-// All are HBM-streaming integer kernels: one field element (32 B) per 256-bit request, one
+// All are HBM-streaming integer kernels: one field element (32 B) per two 128-bit requests, one
 // output index per thread per iteration, grid-stride over a grid sized in multiples of the SM
 // count. No tensor cores (there is no dense contraction on this path).
 #pragma once
@@ -141,13 +141,8 @@ constexpr size_t XCH_TOTAL_BYTES = XCH_ARENA_OFFSET + 2 * XCH_ARENA_HALF;
 
 template <class F>
 __device__ __forceinline__ F ld_elem_cg(const uint64_t* base, size_t idx) {
-    F r;
-    const uint32_t* p = reinterpret_cast<const uint32_t*>(base) + idx * 8;
-    asm volatile("ld.global.cg.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]),
-                   "=r"(r.v[6]), "=r"(r.v[7])
-                 : "l"(p));
-    return r;
+    const uint4* p = reinterpret_cast<const uint4*>(base) + idx * 2;
+    return elem_from<F>(__ldcg(p), __ldcg(p + 1));
 }
 
 // Thread 0 of the finishing block: write the K totals, then (host-mapped mode) raise the flag.
@@ -308,6 +303,7 @@ __device__ __forceinline__ void fused_pass(const TablePtrs& tp, size_t pairs, co
                                            size_t first, size_t stride, Fr (&acc)[FusedShape<D, SKIP1>::K]) {
     constexpr int K = FusedShape<D, SKIP1>::K;
     constexpr int T = D * P;
+    static_assert(!WEIGHTED || P == 1, "the split-eq weight multiplies the single product term");
     uint32_t* wacc = dsm;                                       // [e][word][tid]
     uint32_t* red = dsm + FusedShape<D, SKIP1>::acc_words(BLOCK);  // block_sum scratch
     const int tid = threadIdx.x;
@@ -388,11 +384,6 @@ __device__ __forceinline__ void fused_pass(const TablePtrs& tp, size_t pairs, co
         const size_t ynext = y1;
         const size_t y2 = (y1 < pairs) ? advance(y1) : pairs;
         prefetch_pair(PIPE ? y2 : y1);
-        Fr wgt;
-        if (WEIGHTED) {
-            const size_t mask = ((size_t)1 << tp.in_bits) - 1;
-            wgt = fp_mul(ld_elem<Fr>(tp.e_out, y >> tp.in_bits), ld_elem<Fr>(tp.e_in, y & mask));
-        }
 #pragma unroll
         for (int k = 0; k < P; ++k) {  // one product term at a time: D tables live in registers
             Fr lo[D], hi[D];
@@ -452,7 +443,9 @@ __device__ __forceinline__ void fused_pass(const TablePtrs& tp, size_t pairs, co
                     }
                 }
             }
-            if (WEIGHTED) {
+            if (WEIGHTED) {  // (P == 1) the weight is formed where it is used: nothing extra is live across the binds
+                const size_t yo = y >> tp.in_bits;
+                const Fr wgt = fp_mul(ld_elem<Fr>(tp.e_out, yo), ld_elem<Fr>(tp.e_in, y - (yo << tp.in_bits)));
                 lo[0] = fp_mul(lo[0], wgt);
                 hi[0] = fp_mul(hi[0], wgt);
             }
@@ -513,7 +506,7 @@ __device__ __forceinline__ void fused_pass(const TablePtrs& tp, size_t pairs, co
         // over the block's threads as plain integers (a column sum is < 2^40; the block total stays far below
         // 2^544: at most P * pairs / gridDim.x products of < 2^512 each), then lane e of warp 0 propagates the carries
         // of value e and reduces ONCE. One reduction per block instead of one per thread: the per-thread
-        // reductions were ~13 % of the instructions a pass issued (ncu, profiles/r01b_ncu_fused_round_kernels.md).
+        // reductions were a large share of the instructions a pass issued.
         uint64_t* colsum = reinterpret_cast<uint64_t*>(red);  // K * 17 u64 <= the 8 * K * 8 words of scratch
         const int lane = tid & 31, warp = tid >> 5, nwarps = (int)blockDim.x >> 5;
         __syncthreads();
@@ -654,15 +647,15 @@ static __global__ void __launch_bounds__(256) eq_expand_kernel(const uint64_t* p
 // equivalents per 8 outputs instead of 8. Every store instruction writes 32 consecutive elements per
 // warp (1 KiB, fully coalesced); 32 B of HBM write per output, no reads beyond the 8 KiB low8 table.
 // One Montgomery product per output is inherent to an eq table (2^n - 1 products for 2^n leaves), so
-// with a full 254-bit point this kernel is bound by the integer pipe (66.8 G mul/s x 32 B = 2.1 TB/s),
+// with a full 254-bit point this kernel is bound by the integer pipe (one Montgomery product per 32 B output),
 // not by HBM.
 // CS: streaming (evict-first) stores - the table is written once and consumed by a LATER kernel; keeping 128 MB+ of
-// it dirty in L2 only evicts what the consumer wants there (A/B: tools/eq_store_probe.py, profiles/).
+// it dirty in L2 only evicts what the consumer wants there (A/B: tools/eq_store_probe.py).
 // LOW3: the three register-expanded variables are the LAST three of the point, so a thread's 8 outputs are
 // CONSECUTIVE (256 B; out[(b << 11) | (t << 3) | k] = prefix[b] * mid8[t] * eq3[k], mid8 over the 8 variables before
 // them) instead of 8 KiB apart. Built to test whether the store pattern explains the 2 x DRAM write traffic ncu
-// reports for this kernel (dram__bytes_write = 2.03 x the table at 2^26): it does not - both layouts, with and
-// without streaming stores, write the same bytes (profiles/r02_eq_store_ab.md); LOW3 is 7 % slower and stays off.
+// reports for this kernel: it does not - both layouts, with and without streaming stores, write the same bytes; LOW3
+// is slower and stays off.
 template <bool HI4, bool CS, bool LOW3 = false>
 __global__ void __launch_bounds__(256) eq_stream_kernel(const uint64_t* prefix, const __grid_constant__ EqVars ev,
                                                         const uint64_t* low8, uint64_t* out) {

@@ -2,8 +2,8 @@
 //
 // A sumcheck has log N sequential Fiat-Shamir round trips (the challenge of round k depends on the round
 // polynomial of round k; the transcript is host-owned, specs/clean-slate-prover.md:579-584). With one launch per
-// round each trip costs launch + ramp + drain + publish (~19 us on top of the pass itself, r01 BENCH) - at 2^22
-// that was 65 % of the whole sumcheck. Here the kernel is launched once per batch (cooperatively: every block is
+// round each trip costs launch + ramp + drain + publish on top of the pass itself - most of a 2^22 sumcheck's
+// short rounds. Here the kernel is launched once per batch (cooperatively: every block is
 // co-resident), and every round is driven through a mailbox in host-mapped pinned memory:
 //
 //   host : writes {actions, challenge} then cmd_seq            (one 64-byte line)
@@ -15,8 +15,8 @@
 //          on a ticket counter
 //   last : the last block to arrive copies the lanes to the mailbox (and zeroes them), resets the ticket and raises
 //          res_seq, which the host spins on. The O(K) serial tail - carry propagation and the Montgomery reduction
-//          of each 544-bit sum - runs on the HOST (jb_wide_lanes_reduce_host): one CPU core does it in ~0.2 us,
-//          one GPU lane needs ~2 us, and it sits on the latency path of every round.
+//          of each 544-bit sum - runs on the HOST (jb_wide_lanes_reduce_host): one CPU core does it far faster than
+//          one GPU lane's dependent multiply chain, and it sits on the latency path of every round.
 //
 // The bind -> next round's reads dependency between DIFFERENT blocks is carried by that same chain
 // (stores -> bar.sync -> fence -> ticket atomic ... res_seq -> host -> cmd_seq -> release/acquire -> bar.sync ->
@@ -309,6 +309,44 @@ __host__ __device__ inline unsigned res_need_blocks(int D, int P, uint64_t len, 
     return need > fin ? need : fin;
 }
 
+// The two bind-only loops of the round loop, out of line for the same reason as resident_pass: inlined, their field
+// arithmetic pushed the round loop's own state into local memory.
+// Terminal bind of one member's T tables: `half` outputs, into the table itself (HighToLow) or its partner (LowToHigh).
+template <int T, int ORDER>
+__device__ __noinline__ void final_bind_pass(uint64_t* const* cur, uint64_t* const* oth, uint64_t half, const BindScalar sc,
+                                             bool hi4, uint64_t first, uint64_t stride) {
+    for (uint64_t i = first; i < half; i += stride) {
+#pragma unroll
+        for (int j = 0; j < T; ++j) {
+            const uint64_t* in = cur[j];
+            const Fr lo = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i : 2 * i);
+            const Fr hi = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i + half : 2 * i + 1);
+            const Fr o = hi4 ? bind_pair<true>(lo, hi, sc) : bind_pair<false>(lo, hi, sc);
+            st_elem(ORDER == ORDER_HIGH_TO_LOW ? cur[j] : oth[j], i, o);
+        }
+    }
+}
+
+// Gather: bind member 0's shard (np outputs per table) and store it into every rank's arena (parity half `par`).
+template <int T, int ORDER>
+__device__ __noinline__ void gather_bind_pass(const ResArgs& a, uint64_t* const* cur, uint64_t np, int G, int par,
+                                              const BindScalar sc, bool hi4, uint64_t first, uint64_t stride) {
+    const uint64_t glen = np * (uint64_t)G;  // the gathered table
+    for (uint64_t i = first; i < np; i += stride) {
+        // LowToHigh shards are contiguous blocks of the global table, HighToLow shards are strided
+        const uint64_t gpos = ORDER == ORDER_LOW_TO_HIGH ? (uint64_t)a.rank * np + i : i * (uint64_t)G + a.rank;
+#pragma unroll
+        for (int j = 0; j < T; ++j) {
+            const uint64_t* in = cur[j];
+            const Fr lo = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i : 2 * i);
+            const Fr hi = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i + np : 2 * i + 1);
+            const Fr o = hi4 ? bind_pair<true>(lo, hi, sc) : bind_pair<false>(lo, hi, sc);
+            for (int g = 0; g < G; ++g)
+                st_elem(a.peer[g] + (XCH_ARENA_OFFSET + (size_t)par * XCH_ARENA_HALF) / 8 + (size_t)j * glen * 4, gpos, o);
+        }
+    }
+}
+
 template <int D, int P, int ORDER>
 __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __grid_constant__ ResArgs a) {
     constexpr int T = D * P;
@@ -401,12 +439,16 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
         }
         if (b == 0 && tid == 0) a.mb->tlog[2 * ((seq - 1) & 63)] = global_timer_ns();
         const unsigned actions = (unsigned)(cmdw >> 16);
-        BindScalar sc;
+        // the bind scalar is re-read from the command line at every call: 8 words fewer live across the out-of-line passes
+        const auto sc = [&]() {
+            BindScalar r;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            sc.w[2 * i] = (uint32_t)s_line[2 + i];
-            sc.w[2 * i + 1] = (uint32_t)(s_line[2 + i] >> 32);
-        }
+            for (int i = 0; i < 4; ++i) {
+                r.w[2 * i] = (uint32_t)s_line[2 + i];
+                r.w[2 * i + 1] = (uint32_t)(s_line[2 + i] >> 32);
+            }
+            return r;
+        };
         const bool hi4 = (s_line[2] | s_line[3]) == 0;  // 125-bit challenge [0,0,lo,hi]: 4-row product
 
         unsigned eff_actions = actions;  // what the member loop below executes (a gather turns its bind into an eval)
@@ -416,21 +458,8 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
             const uint64_t len = s_len[0], np = len / 2;      // np = this rank's bound shard
             const uint64_t glen = np * (uint64_t)G;           // the gathered table
             const ResShape sh = res_shape(np, live);
-            if (b < sh.nblk && tid < (int)sh.tpb) {
-                for (uint64_t i = (uint64_t)b * sh.tpb + tid; i < np; i += (uint64_t)sh.nblk * sh.tpb) {
-                    // LowToHigh shards are contiguous blocks of the global table, HighToLow shards are strided
-                    const uint64_t gpos = ORDER == ORDER_LOW_TO_HIGH ? (uint64_t)a.rank * np + i : i * (uint64_t)G + a.rank;
-#pragma unroll
-                    for (int j = 0; j < T; ++j) {
-                        const uint64_t* in = s_cur[0][j];
-                        const Fr lo = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i : 2 * i);
-                        const Fr hi = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i + np : 2 * i + 1);
-                        const Fr o = hi4 ? bind_pair<true>(lo, hi, sc) : bind_pair<false>(lo, hi, sc);
-                        for (int g = 0; g < G; ++g)
-                            st_elem(a.peer[g] + (XCH_ARENA_OFFSET + (size_t)par * XCH_ARENA_HALF) / 8 + (size_t)j * glen * 4, gpos, o);
-                    }
-                }
-            }
+            if (b < sh.nblk && tid < (int)sh.tpb)
+                gather_bind_pass<T, ORDER>(a, s_cur[0], np, G, par, sc(), hi4, (uint64_t)b * sh.tpb + tid, (uint64_t)sh.nblk * sh.tpb);
             // ---- grid barrier; its last arriver also waits for every peer's shard ------------------------------
             __syncthreads();
             if (tid == 0) {
@@ -489,18 +518,8 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
             if (act == RES_ACT_FINAL) {  // terminal bind: no sweep
                 const uint64_t half = len / 2;
                 const ResShape sh = res_shape(half, live);
-                if (b < sh.nblk && tid < (int)sh.tpb) {
-                    for (uint64_t i = (uint64_t)b * sh.tpb + tid; i < half; i += (uint64_t)sh.nblk * sh.tpb) {
-#pragma unroll
-                        for (int j = 0; j < T; ++j) {
-                            const uint64_t* in = s_cur[m][j];
-                            const Fr lo = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i : 2 * i);
-                            const Fr hi = ld_elem_rw<Fr>(in, ORDER == ORDER_HIGH_TO_LOW ? i + half : 2 * i + 1);
-                            const Fr o = hi4 ? bind_pair<true>(lo, hi, sc) : bind_pair<false>(lo, hi, sc);
-                            st_elem(ORDER == ORDER_HIGH_TO_LOW ? s_cur[m][j] : s_oth[m][j], i, o);
-                        }
-                    }
-                }
+                if (b < sh.nblk && tid < (int)sh.tpb)
+                    final_bind_pass<T, ORDER>(s_cur[m], s_oth[m], half, sc(), hi4, (uint64_t)b * sh.tpb + tid, (uint64_t)sh.nblk * sh.tpb);
                 continue;
             }
             const bool bind = act == RES_ACT_BIND_EVAL;
@@ -523,8 +542,9 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                     tp.static_end = ~(size_t)0;
                     uint64_t* gl = a.st->lanes + m * RES_SLOT_U64;
                     uint64_t* sl = live == 1 ? s_lanes + m * RES_SLOT_U64 : nullptr;
-                    if (bind) thin_pass<P, ORDER, true>(tp, nprime, sc, hi4, dsm, b, nb, gl, sl);
-                    else thin_pass<P, ORDER, false>(tp, nprime, sc, hi4, dsm, b, nb, gl, sl);
+                    // one call site per pass kind: the round loop's state is reloaded after one call, not after each variant
+                    const auto pass = bind ? thin_pass<P, ORDER, true> : thin_pass<P, ORDER, false>;
+                    pass(tp, nprime, sc(), hi4, dsm, b, nb, gl, sl);
                 }
                 continue;
             }
@@ -548,12 +568,9 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                     tp.static_end = ((size_t)pairs / 100 * (size_t)a.static_pct / stride) * stride;
                 uint64_t* gl = a.st->lanes + m * RES_SLOT_U64;
                 uint64_t* sl = live == 1 ? s_lanes + m * RES_SLOT_U64 : nullptr;
-                if (!bind)
-                    resident_pass<D, P, ORDER, false, false>(tp, pairs, sc, dsm, first, stride, gl, sl);
-                else if (hi4)
-                    resident_pass<D, P, ORDER, true, true>(tp, pairs, sc, dsm, first, stride, gl, sl);
-                else
-                    resident_pass<D, P, ORDER, true, false>(tp, pairs, sc, dsm, first, stride, gl, sl);
+                const auto pass = !bind ? resident_pass<D, P, ORDER, false, false>
+                                  : hi4 ? resident_pass<D, P, ORDER, true, true> : resident_pass<D, P, ORDER, true, false>;
+                pass(tp, pairs, sc(), dsm, first, stride, gl, sl);
             }
         }
         if (b == 0 && tid == 0) a.mb->tlog2[4 * ((seq - 1) & 63)] = global_timer_ns();
@@ -594,7 +611,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
         const unsigned ln = s_live_next;
         // A block that is alone (live == 1) is poller AND answerer: its warp 0 goes straight back to polling for the
         // next command while warps 1..7 publish this round's answer - the system-scope fence of the publication
-        // (~2 us over PCIe) then overlaps the poll's PCIe read instead of preceding it. With lookahead the next
+        // (a PCIe round trip) then overlaps the poll's PCIe read instead of preceding it. With lookahead the next
         // command is usually already posted, so this is on the critical path of every short round.
         const bool solo = live == 1;
         if (s_last && !(solo && warp == 0)) {

@@ -1,8 +1,8 @@
 // A/B variant of the eval-only sweep (degree 2, s(1) from the claim): evaluation blocks are STAGED INTO SHARED
 // MEMORY by the TMA unit - cp.async.bulk (1-D bulk copies, SASS UBLKCP) issued by a producer warp and tracked by
-// mbarriers - instead of being loaded by every thread with 256-bit LDGs. BASELINE.json's north_star names "TMA
+// mbarriers - instead of being loaded by every thread with 128-bit LDGs. BASELINE.json's north_star names "TMA
 // staging of evaluation blocks into shared memory"; r01 argued against it without building it. This builds it so the
-// choice is a measurement (tools/tma_ab.py, profiles/r02_tma_ab.md):
+// choice is a measurement (tools/tma_ab.py):
 //   * 8 compute warps + 1 producer warp; a ring of STAGES tiles of TILE = 256 pair indices (one per compute thread);
 //     a tile holds, per table, the TILE pairs' lo and hi elements (LowToHigh: one contiguous 16 KiB run;
 //     HighToLow: two 8 KiB runs);

@@ -31,7 +31,7 @@ def test_header_symbols_exported():
 
 def test_version_and_status_strings():
     lib = _lib.load()
-    assert b"sm_100a" in lib.jb_version()
+    assert b"sm_90a" in lib.jb_version()
     assert b"no CPU fallback" in lib.jb_status_str(_lib.JB_ERR_NO_DEVICE)
 
 

@@ -1,4 +1,4 @@
-"""HyperKZG commit + open timing on one B200 (device-resident SRS and polynomial)."""
+"""HyperKZG commit + open timing on one H100 (device-resident SRS and polynomial)."""
 import json, sys, time, pathlib
 import numpy as np
 ROOT = pathlib.Path(__file__).resolve().parents[1]

@@ -1,4 +1,4 @@
-"""Per-kernel timings on one B200 (CUDA events on the launching stream, warm-up, L2-exceeding
+"""Per-kernel timings on one H100 (CUDA events on the launching stream, warm-up, L2-exceeding
 inputs or explicit flush). Writes gpurun_out/microbench.jsonl. Not the driver's bench (bench.py)."""
 import ctypes
 import json
@@ -18,7 +18,7 @@ from jolt_b200.api import _p
 OUT = ROOT / "gpurun_out"
 OUT.mkdir(exist_ok=True)
 quick = "--quick" in sys.argv
-PEAK = 6585.8
+PEAK = 3350.0  # GB/s, H100 SXM data-sheet HBM3 bandwidth
 try:
     PEAK = json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"]
 except Exception:
@@ -68,7 +68,7 @@ def timed(fn, reps=10, warm=3, flush=True):
 for fld in (0, 1):
     for var, name in ((0, "mul_full"), (1, "mul_hi4"), (2, "addsub")):
         g = ctypes.c_double()
-        sess.check(lib.jb_diag_mul_throughput(sess.h, fld, var, 2000, 148 * 8, ctypes.byref(g)))
+        sess.check(lib.jb_diag_mul_throughput(sess.h, fld, var, 2000, torch.cuda.get_device_properties(0).multi_processor_count * 8, ctypes.byref(g)))
         emit(kind="alu", field="Fr" if fld == 0 else "Fq", op=name, gops=round(g.value, 1))
 
 ch125 = np.array([0, 0, 0x123456789ABCDEF1, 0x0FEDCBA987654321], dtype=np.uint64)

@@ -1,4 +1,4 @@
-"""G1 MSM throughput on one B200 (BASELINE config 3): terms/s at 2^16..2^24, synthetic bases
+"""G1 MSM throughput on one H100 (BASELINE config 3): terms/s at 2^16..2^24, synthetic bases
 (i+1)*G generated on the device, uniform 253-bit scalars resident in HBM; the result is checked
 against the closed form at every size. CPU = the C restatement's Pippenger on all host cores."""
 import json, sys, time, pathlib

@@ -1,4 +1,4 @@
-"""A/B of the degree-2 eval-only sweep (round 0 of the 2^22 m = 2 sumcheck): LDG.256 per thread + software pipelining
+"""A/B of the degree-2 eval-only sweep (round 0 of the 2^22 m = 2 sumcheck): two LDG.128 per element per thread + software pipelining
 (fused_round_kernel) against TMA-staged evaluation blocks (eval2_tma_kernel, cp.async.bulk + mbarrier). Both through the
 C ABI with one launch per round (JB_NO_TAIL) so the kernels can be timed with CUDA events and captured by ncu.
 Usage: python tools/tma_ab.py [log_n]   (run under ncu with -k regex:'eval2_tma|fused_round' for the full captures)"""
@@ -13,7 +13,7 @@ from jolt_b200 import field as F
 
 lg = int(sys.argv[1]) if len(sys.argv) > 1 else 22
 n = 1 << lg
-peak = 6585.8
+peak = 3350.0  # GB/s, H100 SXM data-sheet HBM3 bandwidth
 try:
     peak = json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"]
 except Exception:
