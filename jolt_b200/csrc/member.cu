@@ -5,6 +5,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1113,7 +1114,8 @@ void jb_member_destroy(jb_member* mem) {
 //     a single mailbox command carries every member's action and the shared challenge, the kernel answers
 //     with every member's round sums;
 //   * otherwise every active member's pass is enqueued before the first wait (one result slot per member;
-//     short members through their own small resident kernels), then the results are collected.
+//     short members through their own small resident kernels), then the results are collected - in chunks of
+//     JB_RESULT_SLOTS - 1 members when more are active.
 struct jb_scheduler {
     jb_ctx* ctx;
     std::vector<jb_member*> members;
@@ -1163,6 +1165,8 @@ static int scheduler_begin_run(jb_scheduler* s) {
     if (live.empty()) return JB_ERR_UNSUPPORTED;
     return resident_begin(c, live.data(), (int)live.size());
 }
+
+static int overlapped_rounds(jb_scheduler* s, const jb_round_work* work, size_t n_work, uint64_t* out_evals);
 
 int jb_scheduler_prove_round(jb_scheduler* s, const jb_round_work* work, size_t n_work, uint64_t* out_evals) {
     if (!s || (n_work && (!work || !out_evals))) return JB_ERR_INVALID;
@@ -1223,8 +1227,21 @@ int jb_scheduler_prove_round(jb_scheduler* s, const jb_round_work* work, size_t 
         s->run_failed = true;
     }
     // ---- overlapped: enqueue every member's pass, then collect -----------------------------------------
-    if (n_work >= JB_RESULT_SLOTS) return c->fail(JB_ERR_UNSUPPORTED, "scheduler: too many active members in one round");
+    // Slot 0 serves in-place rounds, so at most JB_RESULT_SLOTS - 1 launched passes can be in flight: larger batches
+    // run in chunks of that many members, each chunk enqueued (into slots 1..) and collected before the next.
     c->quiesce_resident(false);
+    for (size_t base = 0; base < n_work; base += JB_RESULT_SLOTS - 1) {
+        const size_t n_chunk = std::min(n_work - base, (size_t)JB_RESULT_SLOTS - 1);
+        int st = overlapped_rounds(s, work + base, n_chunk, out_evals + base * JB_MAX_EVALS * 4);
+        if (st != JB_OK) return st;
+    }
+    return JB_OK;
+}
+
+// one chunk of the overlapped path: every member's pass is enqueued (member i of the chunk reports into result
+// slot i + 1), then the results are collected
+static int overlapped_rounds(jb_scheduler* s, const jb_round_work* work, size_t n_work, uint64_t* out_evals) {
+    jb_ctx* c = s->ctx;
     enum { VIA_LAUNCH = 0, VIA_RUN = 1 };
     int via[JB_RESULT_SLOTS];
     uint64_t seqs[JB_RESULT_SLOTS];

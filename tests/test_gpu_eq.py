@@ -7,6 +7,7 @@ from jolt_b200 import EqPolynomial
 from oracle import bn254 as O
 from oracle import coracle as C
 from gpu_util import rand_limbs
+import sumcheck_ref as S
 
 pytestmark = pytest.mark.gpu
 
@@ -62,6 +63,17 @@ def test_eq_2pow22(sess, kind):
         r[:, 3] &= np.uint64((1 << 61) - 1)
     if kind == "mixed":
         r[12] = rand_limbs(5, 1)[0]
+    got = EqPolynomial.evals(sess, r).evals()
+    want = C.eq_evals(r, None, threads=C.max_threads())
+    assert (got == want).all()
+
+
+@pytest.mark.parametrize("n", [17, 22])
+@pytest.mark.parametrize("kind", ["full", "challenge"])
+def test_eq_extreme_point_coordinates(sess, n, kind):
+    """coordinates 0, 1, p - 1 and limb-extreme values as full elements, and extreme 125-bit [0,0,lo,hi]
+    challenges, shuffled over the point"""
+    r = S.extreme_point(0xE0E + n, n, kind)
     got = EqPolynomial.evals(sess, r).evals()
     want = C.eq_evals(r, None, threads=C.max_threads())
     assert (got == want).all()

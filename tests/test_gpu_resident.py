@@ -14,6 +14,7 @@ from jolt_b200 import field as F
 from oracle import bn254 as O
 from oracle import coracle as C
 from gpu_util import rand_challenge, rand_full, rand_limbs
+from sumcheck_ref import rand_limbs_full
 
 pytestmark = pytest.mark.gpu
 
@@ -91,6 +92,31 @@ def test_resident_2pow16_vs_c_oracle_every_round(sess, order):
         assert got == want, f"round {rnd}"
         bind = rand_challenge(3000 + rnd) if rnd % 2 else rand_full(3000 + rnd)
     cur = [C.bind(t, bind, order) for t in cur]
+    gpu.finish_rounds(bind)
+    assert gpu.final_evals() == [C.mont_to_ints(t)[0] for t in cur]
+    assert sess.launch_count - l0 == 1      # the whole sumcheck was ONE kernel launch
+
+
+@pytest.mark.parametrize("m", [1, 3, 4])
+@pytest.mark.parametrize("order", [HIGH_TO_LOW, LOW_TO_HIGH])
+def test_resident_2pow18_vs_c_oracle_every_round(sess, m, order):
+    """products of 1, 3 and 4 tables at 2^18 (multi-block passes shrinking to one block) through the resident
+    kernel, every round and the final evaluations against the threaded C oracle, inputs over all of [0, p)."""
+    n = 18
+    thr = C.max_threads()
+    tabs = [rand_limbs_full(0xB218 + 8 * m + j, 1 << n) for j in range(m)]
+    gpu = ProductMember(sess, [Polynomial.new(sess, t) for t in tabs], order)
+    cur = tabs
+    bind = None
+    l0 = sess.launch_count
+    for rnd in range(n):
+        if bind is not None:
+            cur = [C.bind(t, bind, order, thr) for t in cur]
+        want = C.mont_to_ints(C.product_round_evals(cur, m, order, thr))
+        got = gpu.prove_round_evals(bind, rnd, (want[0] + want[1]) % O.R_MOD)
+        assert got == want, f"round {rnd}"
+        bind = rand_challenge(6000 + rnd) if rnd % 2 else rand_limbs_full(6000 + rnd, 1)[0]
+    cur = [C.bind(t, bind, order, thr) for t in cur]
     gpu.finish_rounds(bind)
     assert gpu.final_evals() == [C.mont_to_ints(t)[0] for t in cur]
     assert sess.launch_count - l0 == 1      # the whole sumcheck was ONE kernel launch

@@ -11,6 +11,7 @@ from jolt_b200 import field as F
 from oracle import bn254 as O
 from oracle import coracle as C
 from gpu_util import rand_challenge, rand_limbs
+import sumcheck_ref as S
 
 pytestmark = pytest.mark.gpu
 
@@ -90,30 +91,60 @@ def test_eq_member_in_the_engine_and_errors(sess):
         EqProductMember(sess, [Polynomial.from_ints(sess, tabs[0])], C.ints_to_mont(w[:-1]))
 
 
-def test_eq_member_2pow18_vs_c_oracle(sess):
-    """First rounds at 2^18 against the threaded C oracle (eq table materialised on the oracle side only),
-    then the size-independent property: every round keeps s(0)+s(1)==claim and the final claim factors."""
-    n, m = 18, 2
+def eq_member_vs_c_oracle(sess, tabs, w, order, challenge):
+    """Every round, the final evaluations and eq(w, r) of the split-eq member against the threaded C oracle over
+    the materialised eq table (the oracle's rounds halve, so a run costs about two first rounds)."""
+    n, m = len(w), len(tabs)
     thr = C.max_threads()
-    tabs = [rand_limbs(0xE9 + j, 1 << n) for j in range(m)]
-    w = rand_limbs(0x77, n)
-    gpu = EqProductMember(sess, [Polynomial.new(sess, t) for t in tabs], w)
-    cur = [C.eq_evals(w, None, thr)] + tabs
+    gpu = EqProductMember(sess, [Polynomial.new(sess, t) for t in tabs], w, order=order)
+    cur = [C.eq_evals(w, None, thr)] + list(tabs)
     bind, claim = None, None
     for rnd in range(n):
-        if rnd <= 2:
-            if bind is not None:
-                cur = [C.bind(t, bind, O.LOW_TO_HIGH, thr) for t in cur]
-            want = C.mont_to_ints(C.product_round_evals(cur, m + 1, O.LOW_TO_HIGH, thr))
-            if claim is None:
-                claim = (want[0] + want[1]) % O.R_MOD
-            got = gpu.prove_round_evals(bind, rnd, claim)
-            assert got == want
-        else:
-            got = gpu.prove_round_evals(bind, rnd, claim)
-            assert (got[0] + got[1]) % O.R_MOD == claim
-        bind = rand_challenge(3000 + rnd)
+        if bind is not None:
+            cur = [C.bind(t, bind, order, thr) for t in cur]
+        want = C.mont_to_ints(C.product_round_evals(cur, m + 1, order, thr))
+        if claim is None:
+            claim = (want[0] + want[1]) % O.R_MOD
+        assert (want[0] + want[1]) % O.R_MOD == claim, f"round {rnd}: the oracle's own round check"
+        got = gpu.prove_round_evals(bind, rnd, claim)
+        assert got == want, f"round {rnd}"
+        bind = challenge(rnd)
         claim = UnivariatePoly.from_evals(got).evaluate(F.from_limbs(bind))
+    cur = [C.bind(t, bind, order, thr) for t in cur]
     gpu.finish_rounds(bind)
-    fe = gpu.final_evals()
-    assert gpu.eq_scalar() * fe[0] * fe[1] % O.R_MOD == claim
+    fe = [C.mont_to_ints(t)[0] for t in cur]
+    assert gpu.final_evals() == fe[1:]
+    assert gpu.eq_scalar() == fe[0]
+    assert gpu.eq_scalar() * int(np.prod(gpu.final_evals(), dtype=object)) % O.R_MOD == claim
+    gpu.close()
+
+
+def test_eq_member_2pow18_vs_c_oracle(sess):
+    """all 18 rounds at 2^18 against the threaded C oracle"""
+    n, m = 18, 2
+    tabs = [rand_limbs(0xE9 + j, 1 << n) for j in range(m)]
+    eq_member_vs_c_oracle(sess, tabs, rand_limbs(0x77, n), LOW_TO_HIGH, lambda rnd: rand_challenge(3000 + rnd))
+
+
+@pytest.mark.parametrize("n", [15, 16])
+@pytest.mark.parametrize("m", [1, 2, 3])
+@pytest.mark.parametrize("order", [LOW_TO_HIGH, HIGH_TO_LOW])
+def test_eq_member_extreme_point_every_round_vs_c_oracle(sess, n, m, order):
+    """eq points with coordinates 1, p - 1 and limb-extreme values, tables over all of [0, p), extreme challenges;
+    n odd and even so the inner and outer halves of the split differ in size. A zero eq factor is excluded: s(1) is
+    recovered from the claim by dividing by eq(w_cur, 1) times the bound eq prefix (as the reference's
+    gruen_poly), so a coordinate 0, or challenge 0 against a coordinate 1, is refused (checked below)."""
+    tabs = [S.rand_limbs_full(0xE16 + 10 * m + j, 1 << n) for j in range(m)]
+    w = S.extreme_point(0x3E + n, n, zero=False)
+
+    def challenge(rnd):
+        ch = S.extreme_challenge(rnd, n)
+        return ch if ch.any() else S.EXTREME_CHALLENGES[2]
+    eq_member_vs_c_oracle(sess, tabs, w, order, challenge)
+    # a zero eq factor at the current variable is an error, never a wrong round
+    w0 = w.copy()
+    w0[n - 1 if order == LOW_TO_HIGH else 0] = 0
+    gpu = EqProductMember(sess, [Polynomial.new(sess, t) for t in tabs], w0, order=order)
+    with pytest.raises(jolt_b200.JoltB200Error, match="must be invertible"):
+        gpu.prove_round_evals(None, 0, 1)
+    gpu.close()
