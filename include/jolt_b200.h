@@ -327,6 +327,25 @@ int jb_msm_g1_rows(jb_ctx* ctx, jb_srs bases, const void* scalars, size_t rows, 
                    uint64_t* out_xyz);
 /* Same with the scalars already on the device (a table, e.g. a folded HyperKZG polynomial). */
 int jb_msm_g1_table(jb_ctx* ctx, jb_srs bases, size_t offset, jb_table scalars, size_t n, uint64_t out_xyz[12]);
+/* One-hot row commitments: the tier-1 row commitments of Dory for one-hot polynomials (the RA polynomials,
+ * ra(k, j) = 1 iff cycle j touched address k), straight from their address columns. addr[j] is the address cycle j
+ * touched; the all-ones value of the entry width (0xFF for JB_SCALAR_U8, 0xFFFF for JB_SCALAR_U16) means it touched
+ * none, and its column of the polynomial is zero. Coefficient (k, j) is 1 iff addr[j] == k; K and T are powers of two.
+ * The flat coefficient index is idx = j K + k (JB_ONE_HOT_CYCLE_MAJOR) or k T + j (JB_ONE_HOT_ADDRESS_MAJOR). With the
+ * row width W (a power of two, W <= K T, W <= srs length) the matrix has R = K T / W rows, and
+ *   C_r = sum { bases[idx mod W] : coefficient idx is 1 and idx / W = r }
+ * is the true group sum (complete additions: repeated and coinciding partial sums are exact; an empty row is the
+ * identity). count polynomials of the same T, K, W and layout; columns[p] = T entries of `kind` (JB_SCALAR_U8 or
+ * JB_SCALAR_U16, host memory, borrowed for the call). out_xyz: count x R x 12 limbs, polynomial-major, Jacobian
+ * representatives with the conventions of jb_msm_g1_rows. Errors: JB_ERR_INVALID for an address >= K that is not the
+ * none value (found on the device), an unknown kind or layout, K, T or W not a power of two, W > K T, or a null
+ * pointer; JB_ERR_LENGTH for W > srs length; JB_ERR_UNSUPPORTED when count x R >= 2^32 or T >= 2^31. After an error
+ * out_xyz is unspecified and the context stays usable. count == 0 -> JB_OK. Large calls are split internally (over
+ * the polynomials, or over the rows of one polynomial) so that no pass exceeds 2^28 hot entries. */
+#define JB_ONE_HOT_CYCLE_MAJOR 0
+#define JB_ONE_HOT_ADDRESS_MAJOR 1
+int jb_msm_g1_one_hot_rows(jb_ctx* ctx, jb_srs bases, const void* const* columns, size_t count, int kind, size_t T,
+                           size_t K, size_t row_width, int layout, uint64_t* out_xyz);
 
 /* Batch affine addition: batch_g1_additions_multi_affine (crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150),
  * the one-hot / binary column path of Dory's tier-1 commitments (crates/jolt-dory/src/streaming.rs:68,128,152,201).

@@ -12,6 +12,8 @@ from ._lib import JoltB200Error, load  # noqa: F401
 from .api import (  # noqa: F401
     HIGH_TO_LOW,
     LOW_TO_HIGH,
+    ONE_HOT_LAYOUTS,
+    ONE_HOT_NONE,
     SCALAR_KINDS,
     BatchMember,
     EqPolynomial,

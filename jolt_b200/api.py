@@ -615,6 +615,12 @@ def prove_batch_native(members_desc: list[BatchMember], members: list[ProductMem
 
 
 # ---- G1 / MSM ---------------------------------------------------------------------------------------
+# One-hot address columns (G1Bases.one_hot_rows): the entry value that means "this cycle touched no address" (RAM's
+# None), per column dtype, and the coefficient layouts of include/jolt_b200.h.
+ONE_HOT_NONE = {np.dtype(np.uint8): 0xFF, np.dtype(np.uint16): 0xFFFF}
+ONE_HOT_LAYOUTS = {"cycle_major": 0, "address_major": 1}
+
+
 def g1_jacobian_to_affine(xyz_limbs) -> tuple[int, int] | None:
     """Host normalisation of the ABI's Jacobian result (x = X/Z^2, y = Y/Z^3); None = identity."""
     a = np.ascontiguousarray(xyz_limbs, dtype=np.uint64).reshape(3, 4)
@@ -740,6 +746,31 @@ class G1Bases:
         self.s.check(self.s.lib.jb_msm_g1_rows(self.s.h, self.handle, a.ctypes.data_as(ctypes.c_void_p) if n else None,
                                                rows, n // rows, k, _p(out)))
         return out
+
+    def one_hot_rows(self, columns, K: int, row_width: int, layout: str = "cycle_major") -> np.ndarray:
+        """Dory tier-1 row commitments of one-hot polynomials from their address columns (jb_msm_g1_one_hot_rows).
+        `columns`: one uint8 / uint16 array of T addresses, a list of them, or a 2-D array (one column per row); all of
+        one dtype and length. ONE_HOT_NONE[dtype] marks a cycle that touched no address. Coefficient (k, j) = 1 iff
+        column[j] == k, at flat index j K + k ("cycle_major") or k T + j ("address_major"); row r of width `row_width`
+        sums the bases[idx mod row_width] of its hot indices. Returns (count, R, 12) Jacobian limbs, R = K T / row_width."""
+        if layout not in ONE_HOT_LAYOUTS:
+            raise ValueError(f"one_hot_rows: layout must be one of {sorted(ONE_HOT_LAYOUTS)}")
+        if isinstance(columns, np.ndarray) and columns.ndim == 1:
+            columns = [columns]
+        cols = [np.ascontiguousarray(c) for c in columns]
+        if not cols:
+            return np.zeros((0, 0, 12), dtype=np.uint64)
+        dt = cols[0].dtype
+        if dt not in ONE_HOT_NONE or any(c.dtype != dt or c.ndim != 1 or c.shape != cols[0].shape for c in cols):
+            raise ValueError("one_hot_rows: columns must be 1-D uint8 or uint16 arrays of one dtype and length")
+        T = cols[0].shape[0]
+        rows = K * T // row_width if row_width > 0 and K * T >= row_width else 0
+        out = np.zeros((len(cols), max(rows, 1), 12), dtype=np.uint64)
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.ctypes.data for c in cols])
+        kind = SCALAR_KINDS["u8" if dt == np.uint8 else "u16"]
+        self.s.check(self.s.lib.jb_msm_g1_one_hot_rows(self.s.h, self.handle, ptrs, len(cols), kind, T, K, row_width,
+                                                       ONE_HOT_LAYOUTS[layout], _p(out)))
+        return out[:, :rows]
 
     def batch_add(self, index_sets) -> np.ndarray:
         """batch_g1_additions_multi_affine (crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150): one affine

@@ -19,6 +19,7 @@
 // (mod.rs:205) becomes a one-time normalisation at upload.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -666,6 +667,55 @@ __global__ void __launch_bounds__(128) msm_rows_out_kernel(const uint64_t* win, 
     st_elem(out_xyz, 3 * r + 2, Z);
 }
 
+// ---- one-hot front end (jb_msm_g1_one_hot_rows): the counting sort of a one-hot polynomial's hot coefficients into
+//      Dory rows, straight from its address column. Entry e of a pass is cycle j = e mod T of polynomial
+//      p = p_lo + e / T; its address a sets coefficient (a, j), whose flat index is idx = j K + a (cycle-major) or
+//      a T + j (address-major), in bucket p R + idx / W (its row) at column idx mod W. The pass owns the buckets
+//      [b0, b0 + nb). The none value (all ones of the entry width) and identity bases contribute nothing; any other
+//      address >= K sets *bad. SCATTER = false counts the entries of every bucket into `cursor`; SCATTER = true places
+//      the columns at offsets[bucket] + cursor (the scan has zeroed the cursor), bit 31 clear: nothing is negated.
+//      In address-major layout a skewed column sends whole warps to one row, so equal buckets within a warp take ONE
+//      atomic (match.any), as in msm_scatter_kernel<true>. -----------------------------------------------------------
+template <bool SCATTER>
+__global__ void __launch_bounds__(256) one_hot_sort_kernel(const void* cols, int kind, size_t p_lo, size_t n, int log_t,
+                                                           int log_k, int log_w, int log_r, int address_major, size_t b0,
+                                                           size_t nb, const uint64_t* bases, unsigned int* cursor,
+                                                           const unsigned int* offsets, uint32_t* sorted, unsigned int* bad) {
+    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    bool hot = false;
+    unsigned slot = 0;
+    uint32_t col = 0;
+    if (e < n) {
+        const size_t at = (p_lo << log_t) + e;  // position in the packed columns
+        const uint64_t a = kind == SK_U8 ? ((const uint8_t*)cols)[at] : ((const uint16_t*)cols)[at];
+        const uint64_t none = kind == SK_U8 ? 0xFFu : 0xFFFFu;
+        if (a != none) {
+            if (a >> log_k) {
+                if (!SCATTER) atomicOr(bad, 1u);
+            } else {
+                const uint64_t j = at & (((uint64_t)1 << log_t) - 1);
+                const uint64_t idx = address_major ? (a << log_t) | j : (j << log_k) | a;
+                const uint64_t bucket = ((uint64_t)(at >> log_t) << log_r) + (idx >> log_w);
+                col = (uint32_t)(idx & (((uint64_t)1 << log_w) - 1));
+                if (bucket >= b0 && bucket - b0 < nb) {
+                    slot = (unsigned)(bucket - b0);
+                    hot = !(ld_elem<Fq>(bases, 2 * (size_t)col).is_zero() && ld_elem<Fq>(bases, 2 * (size_t)col + 1).is_zero());
+                }
+            }
+        }
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, hot);
+    if (!hot) return;
+    const unsigned peers = __match_any_sync(m, slot);
+    const int leader = __ffs(peers) - 1;
+    unsigned int base = 0;
+    if (lane == leader) base = atomicAdd(&cursor[slot], (unsigned)__popc(peers));
+    if (!SCATTER) return;
+    base = __shfl_sync(peers, base, leader);
+    sorted[offsets[slot] + base + (unsigned)__popc(peers & ((1u << lane) - 1u))] = col;
+}
+
 // ---- binary columns: msm_binary (the `all(s <= 1)` arm of VariableBaseMSM::msm / msm_u8,
 //      crates/jolt-prover-legacy/src/msm/mod.rs:35-47, 96-106). The result is the plain sum of the selected bases: no
 //      digits, no sort - every thread walks its own 16-flag groups and adds the selected bases into ONE XYZZ
@@ -835,6 +885,43 @@ bool canonical_q(const uint64_t* a) {
 
 using Guard = CtxGuard;
 
+// 2. the exclusive scans of the histogram `hist` (nb counters): bucket offsets, task offsets, and the histogram zeroed
+// into the scatter cursor. block_sums: 2 x 1024 counters (nb <= 4 Mi).
+void launch_bucket_scan(jb_ctx* c, unsigned int* hist, unsigned int* offsets, unsigned int* toff, size_t nb,
+                        unsigned int* block_sums, unsigned maxq, unsigned pad_shift) {
+    const unsigned scan_blocks = (unsigned)((nb + SCAN_PER_BLOCK - 1) / SCAN_PER_BLOCK);
+    msm_scan_local_kernel<<<scan_blocks, 1024, 0, c->stream>>>(hist, offsets, toff, nb, block_sums, maxq, pad_shift);
+    msm_scan_blocks_kernel<<<1, 1024, 0, c->stream>>>(block_sums, (int)scan_blocks, offsets, toff, nb);
+    msm_scan_apply_kernel<<<scan_blocks, 1024, 0, c->stream>>>(offsets, toff, nb, block_sums);
+    c->launches += 3;
+}
+
+// 4. once the sorted lists exist: the task plan in length order, the bucket accumulation and the fold of split buckets
+// into `buckets` (nb XYZZ points; an empty bucket becomes the identity). shift == 0: `src` is the affine base array
+// gathered through `sorted`; shift = L > 0: `src` holds the level-L points of the batched-affine levels. `len_hist` is
+// zero on entry; the timed range `tix` (ctx timing_begin) ends after the accumulation.
+void launch_bucket_accumulate(jb_ctx* c, const uint64_t* src, const uint32_t* sorted, const unsigned int* offsets,
+                              const unsigned int* toff, size_t nb, size_t max_tasks, unsigned maxq, unsigned shift,
+                              unsigned int* len_hist, uint32_t* task_bucket, uint32_t* order, uint64_t* buckets,
+                              uint64_t* partial, int tix) {
+    msm_len_hist_kernel<<<MSM_TASK_BLOCKS, 256, 0, c->stream>>>(offsets, toff, nb, maxq, len_hist, shift);
+    msm_tasks_kernel<<<MSM_TASK_BLOCKS, 256, 0, c->stream>>>(offsets, toff, nb, maxq, len_hist, task_bucket, order, shift);
+    const unsigned blocks = (unsigned)((max_tasks + 127) / 128);
+    if (shift)
+        msm_accumulate_kernel<true><<<blocks, 128, 0, c->stream>>>(src, sorted, offsets, toff, task_bucket, order, nb, buckets,
+                                                                   partial, maxq, shift);
+    else
+        msm_accumulate_kernel<false><<<blocks, 128, 0, c->stream>>>(src, sorted, offsets, toff, task_bucket, order, nb, buckets,
+                                                                    partial, maxq, 0u);
+    c->timing_end(tix);
+    msm_combine_kernel<<<(unsigned)((nb + 127) / 128), 128, 0, c->stream>>>(toff, nb, partial, buckets);
+    c->launches += 4;
+    if (plan_cap(maxq) > MSM_MAX_CHUNKS) {
+        msm_combine_wide_kernel<<<(unsigned)nb, 256, 0, c->stream>>>(toff, partial, buckets);
+        c->launches++;
+    }
+}
+
 // `srs`: the resident bases; terms are bases[offset .. offset + n).
 // rows > 1 (jb_msm_g1_rows): n = rows * row_w terms, row r = scalars[r * row_w ..) against bases[0 .. row_w); the
 // small table (8-bit shared windows) must cover row_w; out_xyz receives rows x 12 limbs.
@@ -898,7 +985,6 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
     uint32_t *digits = nullptr, *sorted = nullptr, *task_bucket = nullptr, *order = nullptr;
     unsigned int* len_hist = nullptr;
     unsigned int *hist = nullptr, *offsets = nullptr, *toff = nullptr, *block_sums = nullptr;
-    const unsigned scan_blocks = (unsigned)((nb + SCAN_PER_BLOCK - 1) / SCAN_PER_BLOCK);  // <= 512 (c <= 22)
     uint64_t *buckets = nullptr, *partial = nullptr, *seg = nullptr, *win = nullptr, *d_out = nullptr;
     uint64_t *tree_a = nullptr, *tree_b = nullptr;
     const size_t tree_pts = (size_t)Weff * ((p.T + 2047) / 2048) + 1;
@@ -933,9 +1019,7 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
             msm_digits_kernel<true><<<g, 256, 0, c->stream>>>(d_scalars, kind, d_bases, n, p.c, p.W, p.B, shared ? 1 : 0, digits, hist, row_w, halving);
         else
             msm_digits_kernel<false><<<g, 256, 0, c->stream>>>(d_scalars, kind, d_bases, n, p.c, p.W, p.B, shared ? 1 : 0, digits, hist, row_w, halving);
-        msm_scan_local_kernel<<<scan_blocks, 1024, 0, c->stream>>>(hist, offsets, toff, nb, block_sums, maxq, ba_levels);
-        msm_scan_blocks_kernel<<<1, 1024, 0, c->stream>>>(block_sums, (int)scan_blocks, offsets, toff, nb);
-        msm_scan_apply_kernel<<<scan_blocks, 1024, 0, c->stream>>>(offsets, toff, nb, block_sums);
+        launch_bucket_scan(c, hist, offsets, toff, nb, block_sums, maxq, ba_levels);  // nb <= 4 Mi
         {   // scatter, ordered in time by destination region once the destination outgrows the L2 (see the kernel)
             int mode = 0, regions = 1;
             unsigned range_shift = 0;
@@ -977,21 +1061,8 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
             c->launches++;
             acc_src = dst;
         }
-        msm_len_hist_kernel<<<MSM_TASK_BLOCKS, 256, 0, c->stream>>>(offsets, toff, nb, maxq, len_hist, ba_levels);
-        msm_tasks_kernel<<<MSM_TASK_BLOCKS, 256, 0, c->stream>>>(offsets, toff, nb, maxq, len_hist, task_bucket, order, ba_levels);
-        c->launches++;
-        if (ba_levels)
-            msm_accumulate_kernel<true><<<(unsigned)((max_tasks + 127) / 128), 128, 0, c->stream>>>(acc_src, sorted, offsets, toff, task_bucket,
-                                                                                                order, nb, buckets, partial, maxq, ba_levels);
-        else
-            msm_accumulate_kernel<false><<<(unsigned)((max_tasks + 127) / 128), 128, 0, c->stream>>>(d_gather, sorted, offsets, toff, task_bucket,
-                                                                                                 order, nb, buckets, partial, maxq, 0u);
-        c->timing_end(tix);
-        msm_combine_kernel<<<(unsigned)((nb + 127) / 128), 128, 0, c->stream>>>(toff, nb, partial, buckets);
-        if (plan_cap(maxq) > MSM_MAX_CHUNKS) {
-            msm_combine_wide_kernel<<<(unsigned)nb, 256, 0, c->stream>>>(toff, partial, buckets);
-            c->launches++;
-        }
+        launch_bucket_accumulate(c, acc_src, sorted, offsets, toff, nb, max_tasks, maxq, ba_levels, len_hist, task_bucket, order,
+                                 buckets, partial, tix);
         msm_segment_kernel<<<(unsigned)(((size_t)Weff * p.T + 127) / 128), 128, 0, c->stream>>>(buckets, Weff, p.B, p.T, msm_seg_size(p.B), seg);
         {   // tree-sum the T segment points of every bucket set, ping-ponging between two scratch buffers
             const uint64_t* src = seg;
@@ -1013,7 +1084,7 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
         }
         if (by_rows) msm_rows_out_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, c->stream>>>(win, rows, d_out);
         else msm_final_kernel<<<1, 32, 0, c->stream>>>(win, Weff, d_out);
-        c->launches += 10;
+        c->launches += 4;  // digits, scatter, segments, output (the scan and accumulation helpers count their own)
         st = c->check(cudaGetLastError(), "msm kernels");
     }
     if (by_rows) {
@@ -1043,6 +1114,95 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
     c->dev_free(tree_a);
     c->dev_free(tree_b);
     c->dev_free(d_out);
+    return st;
+}
+
+// One-hot row commitments (jb_msm_g1_one_hot_rows, arguments validated): the `count` address columns of T = 2^log_t
+// entries go to the device in one buffer; the count x R buckets (polynomial, row) are then committed in passes, each
+// one counting sort (one_hot_sort_kernel), the scans and the accumulation of jb_msm_g1_rows' pipeline over the plain
+// affine bases, and the XYZZ -> Jacobian conversion of every bucket. A pass keeps to <= 2^28 hot entries (32-bit
+// sorted positions, and the workspace jb_msm_g1_rows keeps to) and <= 4 Mi buckets (the scan): a polynomial holds at
+// most T hot entries and a row at most W, so a pass covers whole polynomials, or a row range of one polynomial when a
+// single polynomial exceeds either bound.
+int one_hot_device(jb_ctx* c, const Srs& srs, const void* const* columns, size_t count, int kind, int log_t, int log_k,
+                   int log_w, int address_major, uint64_t* out_xyz) {
+    constexpr int LOG_PASS_ENTRIES = 28, LOG_PASS_BUCKETS = 22;
+    const int log_r = log_k + log_t - log_w;
+    const size_t T = (size_t)1 << log_t, R = (size_t)1 << log_r, total = count << log_r;
+    size_t step, cap;  // buckets per pass (whole polynomials, or a power of two below R), hot entries per pass (bound)
+    if (log_t <= LOG_PASS_ENTRIES && log_r <= LOG_PASS_BUCKETS) {
+        const size_t polys = std::min(count, (size_t)1 << std::min(LOG_PASS_ENTRIES - log_t, LOG_PASS_BUCKETS - log_r));
+        step = polys << log_r;
+        cap = polys << log_t;
+    } else {
+        step = (size_t)1 << std::min(LOG_PASS_BUCKETS, std::max(0, LOG_PASS_ENTRIES - log_w));
+        cap = std::min(step << log_w, T);
+    }
+    // a row holds at most W entries: rows wider than 64 chunks of MSM_CHUNK take the small-kind cap and the wide fold
+    const size_t W = (size_t)1 << log_w;
+    const unsigned maxq = W > (size_t)MSM_CHUNK * MSM_MAX_CHUNKS ? MSM_MAX_CHUNKS_SMALL : MSM_MAX_CHUNKS;
+    const size_t max_tasks = step + cap / MSM_CHUNK + 1;
+    const size_t esz = (size_t)small_kind_bytes(kind);
+    void* d_cols = nullptr;
+    uint32_t *sorted = nullptr, *task_bucket = nullptr, *order = nullptr;
+    unsigned int *hist = nullptr, *offsets = nullptr, *toff = nullptr, *block_sums = nullptr, *len_hist = nullptr, *d_bad = nullptr;
+    uint64_t *buckets = nullptr, *partial = nullptr, *d_out = nullptr;
+    int st = c->dev_alloc(&d_cols, count * T * esz);
+    for (size_t p = 0; p < count && st == JB_OK; ++p)
+        st = c->check(cudaMemcpyAsync((char*)d_cols + p * T * esz, columns[p], T * esz, cudaMemcpyHostToDevice, c->stream),
+                      "one_hot_rows columns H2D");
+    if (st == JB_OK) st = c->dev_alloc((void**)&sorted, cap * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&hist, step * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&offsets, (step + 1) * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&toff, (step + 1) * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&block_sums, 2 * 1024 * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&task_bucket, max_tasks * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&order, max_tasks * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&len_hist, 2 * MSM_LEN_BINS * 4);
+    if (st == JB_OK) st = c->dev_alloc((void**)&buckets, step * 128);
+    if (st == JB_OK) st = c->dev_alloc((void**)&partial, max_tasks * 128);
+    if (st == JB_OK) st = c->dev_alloc((void**)&d_out, step * 96);
+    if (st == JB_OK) st = c->dev_alloc((void**)&d_bad, 4);
+    if (st == JB_OK) st = c->check(cudaMemsetAsync(d_bad, 0, 4, c->stream), "one_hot_rows memset");
+    for (size_t b0 = 0; b0 < total && st == JB_OK; b0 += step) {
+        const size_t nb = std::min(step, total - b0);
+        const size_t p_lo = b0 >> log_r, p_hi = (b0 + nb + R - 1) >> log_r;
+        const size_t n = (p_hi - p_lo) << log_t;
+        const unsigned g = (unsigned)((n + 255) / 256);
+        st = c->check(cudaMemsetAsync(hist, 0, nb * 4, c->stream), "one_hot_rows memset");
+        if (st == JB_OK) st = c->check(cudaMemsetAsync(len_hist, 0, 2 * MSM_LEN_BINS * 4, c->stream), "one_hot_rows memset");
+        if (st != JB_OK) break;
+        one_hot_sort_kernel<false><<<g, 256, 0, c->stream>>>(d_cols, kind, p_lo, n, log_t, log_k, log_w, log_r, address_major, b0,
+                                                             nb, srs.xy, hist, nullptr, nullptr, d_bad);
+        launch_bucket_scan(c, hist, offsets, toff, nb, block_sums, maxq, 0);
+        one_hot_sort_kernel<true><<<g, 256, 0, c->stream>>>(d_cols, kind, p_lo, n, log_t, log_k, log_w, log_r, address_major, b0,
+                                                            nb, srs.xy, hist, offsets, sorted, d_bad);
+        const int tix = c->timing_begin(4, n, 0);
+        launch_bucket_accumulate(c, srs.xy, sorted, offsets, toff, nb, max_tasks, maxq, 0, len_hist, task_bucket, order, buckets,
+                                 partial, tix);
+        msm_rows_out_kernel<<<(unsigned)((nb + 127) / 128), 128, 0, c->stream>>>(buckets, nb, d_out);
+        c->launches += 3;
+        st = c->check(cudaGetLastError(), "one_hot_rows kernels");
+        if (st == JB_OK)
+            st = c->check(cudaMemcpyAsync(out_xyz + 12 * b0, d_out, nb * 96, cudaMemcpyDeviceToHost, c->stream), "one_hot_rows D2H");
+    }
+    if (st == JB_OK) st = c->check(cudaMemcpyAsync(c->h_small, d_bad, 4, cudaMemcpyDeviceToHost, c->stream), "one_hot_rows flag D2H");
+    if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "one_hot_rows sync");
+    if (st == JB_OK && *(const unsigned int*)c->h_small)
+        st = c->fail(JB_ERR_INVALID, "one_hot_rows: an address is >= K and not the none value");
+    c->dev_free(d_cols);
+    c->dev_free(sorted);
+    c->dev_free(hist);
+    c->dev_free(offsets);
+    c->dev_free(toff);
+    c->dev_free(block_sums);
+    c->dev_free(task_bucket);
+    c->dev_free(order);
+    c->dev_free(len_hist);
+    c->dev_free(buckets);
+    c->dev_free(partial);
+    c->dev_free(d_out);
+    c->dev_free(d_bad);
     return st;
 }
 
@@ -1401,6 +1561,37 @@ int jb_msm_g1_rows(jb_ctx* c, jb_srs h, const void* scalars, size_t rows, size_t
         if (d_s) c->dev_free(d_s);
     }
     return st;
+}
+
+int jb_msm_g1_one_hot_rows(jb_ctx* c, jb_srs h, const void* const* columns, size_t count, int kind, size_t T, size_t K,
+                           size_t row_width, int layout, uint64_t* out_xyz) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    auto pow2 = [](size_t x) { return x != 0 && (x & (x - 1)) == 0; };
+    auto log2_of = [](size_t x) {
+        int l = 0;
+        while (x >> (l + 1)) ++l;
+        return l;
+    };
+    if (kind != SK_U8 && kind != SK_U16) return c->fail(JB_ERR_INVALID, "one_hot_rows: addresses must be JB_SCALAR_U8 or JB_SCALAR_U16");
+    if (layout != JB_ONE_HOT_CYCLE_MAJOR && layout != JB_ONE_HOT_ADDRESS_MAJOR) return c->fail(JB_ERR_INVALID, "one_hot_rows: unknown layout");
+    if (!pow2(T) || !pow2(K)) return c->fail(JB_ERR_INVALID, "one_hot_rows: K and T must be powers of two");
+    const int log_t = log2_of(T), log_k = log2_of(K);
+    if (log_t >= 31 || log_k + log_t > 62) return c->fail(JB_ERR_UNSUPPORTED, "one_hot_rows: T must be < 2^31 and K T <= 2^62");
+    if (!pow2(row_width) || log2_of(row_width) > log_k + log_t)
+        return c->fail(JB_ERR_INVALID, "one_hot_rows: the row width must be a power of two <= K T");
+    if (count == 0) return JB_OK;
+    if (!columns || !out_xyz) return c->fail(JB_ERR_INVALID, "one_hot_rows: null pointer");
+    for (size_t p = 0; p < count; ++p)
+        if (!columns[p]) return c->fail(JB_ERR_INVALID, "one_hot_rows: null column");
+    const int log_w = log2_of(row_width), log_r = log_k + log_t - log_w;
+    Guard g(c);
+    auto it = c->srs.find(h);
+    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
+    if (row_width > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
+    if (log_r >= 32 || count >= ((size_t)1 << (32 - log_r)))
+        return c->fail(JB_ERR_UNSUPPORTED, "one_hot_rows: count x R must be < 2^32");
+    return one_hot_device(c, it->second, columns, count, kind, log_t, log_k, log_w, layout == JB_ONE_HOT_ADDRESS_MAJOR ? 1 : 0,
+                          out_xyz);
 }
 
 int jb_msm_g1_device(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* d_scalars, size_t n, uint64_t out_xyz[12]) {
