@@ -198,6 +198,7 @@ static int ctx_create_impl(int device, bool borrow, void* cuda_stream, jb_ctx** 
     if (const char* ml = std::getenv("JB_RESIDENT_MAX_LOG")) c->resident_max_log = std::atoi(ml);
     if (const char* sp = std::getenv("JB_STATIC_PCT")) c->resident_static_pct = std::max(0, std::min(100, std::atoi(sp)));
     if (const char* ts = std::getenv("JB_RESIDENT_TIMEOUT_S")) c->resident_timeout_cycles = (long long)(std::atof(ts) * 1.9e9);
+    if (const char* rs = std::getenv("JB_RES_STAGED")) c->res_staged = std::atoi(rs) != 0;
     if (std::getenv("JB_EVAL_TMA")) c->eval_tma = true;
     if (std::getenv("JB_NO_LOOKAHEAD")) c->lookahead = false;
     if (const char* es = std::getenv("JB_EQ_STORE")) c->eq_store_mode = std::atoi(es);

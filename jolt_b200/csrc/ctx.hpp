@@ -84,6 +84,7 @@ struct jb_ctx {
     int eq_layout = 0;              // eq stream kernel: 0 = a warp writes 1 KiB runs (a thread's outputs 8 KiB apart), 1 = a thread's 8 outputs consecutive
     int eq_store_mode = -1;         // eq table stores: -1 auto, 0 default caching, 1 streaming (evict-first)
     int resident_static_pct = 75;  // big resident passes: statically laid-out share of the range (JB_STATIC_PCT; 100 = all)
+    bool res_staged = true;         // resident D = 2 products: large passes staged through shared memory (JB_RES_STAGED=0: off)
     long long resident_timeout_cycles = 20000000000LL;  // a resident kernel gives its SMs back after this long without a command
     bool lookahead = true;          // answer thin rounds from the previous answer's lookahead sums (JB_NO_LOOKAHEAD: off)
     int resident_max_log = 40;      // a member may enter resident service when log2(len) <= this (JB_RESIDENT_MAX_LOG)

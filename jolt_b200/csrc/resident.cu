@@ -25,13 +25,16 @@ ResKernel pick_order(int order) {
 }
 
 // The instantiated shapes: plain products of 1..4 tables and the two-term degree-2 sum of products
-// (IncClaimReduction: A * RamInc + B * RdInc).
-ResKernel pick_kernel(int D, int P, int order, size_t* smem) {
+// (IncClaimReduction: A * RamInc + B * RdInc). `staged`: the D = 2, P = 1 kernel runs its large passes as
+// staged_pass, whose ring of shared-memory stages is larger than resident_pass's accumulators.
+ResKernel pick_kernel(int D, int P, int order, bool staged, size_t* smem) {
     *smem = 0;
     if (P == 1) {
         switch (D) {
             case 1: *smem = FusedShape<1, true>::smem_bytes(RES_BLOCK); return pick_order<1, 1>(order);
-            case 2: *smem = FusedShape<2, true>::smem_bytes(RES_BLOCK); return pick_order<2, 1>(order);
+            case 2:
+                *smem = std::max(FusedShape<2, true>::smem_bytes(RES_BLOCK), staged ? (size_t)STG_SMEM_BYTES : (size_t)0);
+                return pick_order<2, 1>(order);
             case 3: *smem = FusedShape<3, true>::smem_bytes(RES_BLOCK); return pick_order<3, 1>(order);
             case 4: *smem = FusedShape<4, true>::smem_bytes(RES_BLOCK); return pick_order<4, 1>(order);
             default: return nullptr;
@@ -46,15 +49,23 @@ ResKernel pick_kernel(int D, int P, int order, size_t* smem) {
 
 // occupancy of a shape (cached): also forces the module to load before any resident kernel is alive
 int kernel_blocks_per_sm(ResKernel k, size_t smem) {
+    struct Entry {
+        ResKernel k;
+        size_t smem;
+        int nb;
+    };
     static std::mutex mu;
-    static std::vector<std::pair<ResKernel, int>> cache;
+    static std::vector<Entry> cache;
     std::lock_guard<std::mutex> lk(mu);
-    for (auto& kv : cache)
-        if (kv.first == k) return kv.second;
-    cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    size_t attr = smem;  // the attribute is per function: never below a size another context launches it with
+    for (auto& e : cache) {
+        if (e.k == k && e.smem == smem) return e.nb;
+        if (e.k == k) attr = std::max(attr, e.smem);
+    }
+    cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attr);
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, (const void*)k, RES_BLOCK, smem) != cudaSuccess || nb < 1) nb = 1;
-    cache.emplace_back(k, nb);
+    cache.push_back({k, smem, nb});
     return nb;
 }
 
@@ -156,7 +167,7 @@ bool resident_eligible(const jb_member* mem) {
     while (((size_t)1 << lg) < mem->len) ++lg;
     if ((int)lg > mem->ctx->resident_max_log) return false;
     size_t smem;
-    return pick_kernel(mem->m, mem->terms, mem->order, &smem) != nullptr;
+    return pick_kernel(mem->m, mem->terms, mem->order, mem->ctx->res_staged, &smem) != nullptr;
 }
 
 bool jb_ctx::has_exclusive_run() const {
@@ -179,7 +190,8 @@ int resident_begin(jb_ctx* c, jb_member** mems, int n, uint64_t first_len, bool 
         if (m->ctx != c || m->m != D || m->terms != P || m->order != order || !resident_eligible(m)) return JB_ERR_UNSUPPORTED;
     }
     size_t smem = 0;
-    ResKernel kernel = pick_kernel(D, P, order, &smem);
+    const bool staged = c->res_staged && D == 2 && P == 1;
+    ResKernel kernel = pick_kernel(D, P, order, staged, &smem);
     if (!kernel) return JB_ERR_UNSUPPORTED;
     const int per_sm = kernel_blocks_per_sm(kernel, smem);
     const unsigned cap = (unsigned)(c->sm_count * per_sm);
@@ -233,6 +245,7 @@ int resident_begin(jb_ctx* c, jb_member** mems, int n, uint64_t first_len, bool 
     args.st = (ResState*)run->res.d_state;
     args.timeout_cycles = c->resident_timeout_cycles;
     args.static_pct = c->resident_static_pct;  // ~10 s of SM clocks without a command: give the SMs back
+    args.staged = staged;
     args.world = c->world;
     args.rank = c->rank;
     for (int g = 0; g < 16; ++g) args.peer[g] = c->xch_peer[g];

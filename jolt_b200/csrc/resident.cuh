@@ -32,6 +32,7 @@
 // raises a flag per peer, waits for the peers' flags in its own buffer and sums - before the totals go to the
 // host. No NCCL launch, no extra kernel (comm.cu owns the buffers).
 #pragma once
+#include "bulk_copy.cuh"
 #include "poly_kernels.cuh"
 
 namespace jb {
@@ -117,6 +118,7 @@ struct ResArgs {
     ResState* st;       // device
     long long timeout_cycles;
     int static_pct;     // big passes: this share of the pair range is laid out statically, the rest is claimed (100 = off)
+    int staged;         // D = 2, P = 1: large passes run staged_pass (dynamic shared memory >= STG_SMEM_BYTES)
     // peer exchange (world > 1): exchange buffer of every rank as mapped in THIS process
     uint64_t* peer[16];
     int world, rank;
@@ -287,6 +289,193 @@ __device__ __noinline__ void thin_pass(const TablePtrs tp, uint64_t nprime, cons
     }
 }
 
+// ---- staged pass (D = 2, P = 1, more than RES_THIN_PAIRS pairs) ------------------------------------------------
+// resident_pass is bound by HBM, yet a thread there issues its loads, waits for them and only then multiplies: while
+// a block multiplies it has no table reads in flight, so loads and arithmetic add up instead of overlapping. Here the
+// tables are brought into a ring of STG_STAGES shared-memory stages by the bulk-copy unit (cp.async.bulk, completion
+// counted on one mbarrier per stage). Thread 0 refills a stage with the tile STG_STAGES ahead as soon as the block has
+// read it out, so while the block binds and multiplies, the next STG_STAGES tiles are on their way.
+//   tile      : STG_TILE consecutive pair indices y0 .., both tables; EPP elements per pair and table (4 with a bind)
+//   LowToHigh : a pair's elements are contiguous; a table's part of a tile is four runs of 32 pairs, placed 16 B
+//               further apart in shared memory than their length
+//   HighToLow : EPP runs of STG_TILE elements at y0 + u * pairs (u < EPP); table 1's part sits 16 B off a 128 B line
+// With those offsets the eight threads of each quarter warp read 8 distinct bank groups with their 128-bit loads.
+// Two threads serve a pair: thread j = tid & 1 binds table j's lo and hi, the two swap one value with a shuffle, then
+// the even thread accumulates lo0 lo1 (s(0)) and the odd one (hi0 - lo0)(hi1 - lo1) (s(inf)) - the same products as
+// resident_pass, into a 17-word REGISTER accumulator, summed over each warp with REDUX at the end (as thin_pass).
+// Work: tiles below static_end are dealt round robin (b, b + nblk, ..), the rest is claimed a tile at a time from
+// *tp.work; a claimed tile is always consumed in full.
+constexpr int STG_TILE = 128;
+constexpr int STG_STAGES = 2;
+constexpr uint32_t STG_STAGE_BYTES = 2 * (STG_TILE * 4 * 32 + 128);  // two tables x 4 elements per pair + the offsets
+constexpr uint32_t STG_BAR_OFF = STG_STAGES * STG_STAGE_BYTES;        // mbarriers [STG_STAGES], then tile ids
+constexpr uint32_t STG_RED_OFF = STG_BAR_OFF + STG_STAGES * 16;      // per-warp column sums [8 warps][2 x 17]
+constexpr uint32_t STG_SMEM_BYTES = STG_RED_OFF + (RES_BLOCK / 32) * 2 * 17 * 8;
+constexpr uint32_t STG_NONE = 0xffffffffu;
+// The cooperative grid is sm_count x (blocks per SM from the occupancy query): a shared-memory budget that allowed
+// only one block per SM would halve it without any error. Static part: a bound on the __shared__ arrays of
+// resident_rounds_kernel<2, 1, *> (ptxas -v reports 9216 B; tests/test_build_artifacts_staged.py holds it to this).
+constexpr size_t RES_STATIC_SMEM_D2 = 10 * 1024;
+static_assert(STG_SMEM_BYTES + RES_STATIC_SMEM_D2 <= 113 * 1024, "two resident blocks per SM (228 KB)");
+
+__device__ __forceinline__ Fr lds_fr(uint32_t addr) {
+    Fr r;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]) : "r"(addr));
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4+16];" : "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7]) : "r"(addr));
+    return r;
+}
+__device__ __forceinline__ void stg_fr(uint64_t* base, size_t idx, const Fr& x) {
+    uint32_t* p = reinterpret_cast<uint32_t*>(base) + idx * 8;
+    asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(x.v[0]), "r"(x.v[1]), "r"(x.v[2]), "r"(x.v[3]) : "memory");
+    asm volatile("st.global.v4.u32 [%0+16], {%1,%2,%3,%4};" ::"l"(p), "r"(x.v[4]), "r"(x.v[5]), "r"(x.v[6]), "r"(x.v[7]) : "memory");
+}
+
+template <int ORDER, bool BIND, bool HI4>
+__device__ __noinline__ void staged_pass(const TablePtrs tp, size_t pairs, const BindScalar sc, uint8_t* smem, unsigned b,
+                                         unsigned nblk, uint32_t static_end, uint64_t* g_lanes, uint64_t* s_dst) {
+    constexpr int EPP = BIND ? 4 : 2;
+    constexpr uint32_t SUB = 32 * EPP * 32;  // LowToHigh: one run of 32 pairs
+    constexpr uint32_t TOFF = ORDER == ORDER_LOW_TO_HIGH ? 4 * SUB + 64 : EPP * STG_TILE * 32 + 16;  // table 1's part
+    constexpr uint32_t ESTEP = ORDER == ORDER_LOW_TO_HIGH ? 32 : STG_TILE * 32;  // between a thread's elements
+    static_assert(2 * TOFF <= STG_STAGE_BYTES, "a tile overflows its stage");
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, j = tid & 1;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + STG_BAR_OFF);
+    uint32_t* tile_id = reinterpret_cast<uint32_t*>(bar + STG_STAGES);
+    const uint32_t ntiles = (uint32_t)(pairs / STG_TILE);
+    int p;         // this thread's pair within a tile
+    uint32_t off;  // and the offset of its first element in a stage
+    if (ORDER == ORDER_LOW_TO_HIGH) {
+        const int q = (tid >> 1) & 3, r = tid >> 3;
+        p = q * 32 + r;
+        off = j * TOFF + q * (SUB + 16) + r * EPP * 32;
+    } else {
+        p = tid >> 1;
+        off = j * TOFF + p * 32;
+    }
+
+    uint32_t next = b;  // thread 0: the next tile of the static part
+    bool dyn = false, done = false;
+    const auto produce = [&](int s) {
+        uint32_t t = STG_NONE;
+        if (!done) {
+            if (!dyn && next < static_end) {
+                t = next;
+                next += nblk;
+            } else {
+                dyn = true;
+                if (static_end < ntiles) {
+                    const uint32_t c = static_end + atomicAdd(tp.work, 1u);
+                    if (c < ntiles) t = c;
+                }
+            }
+            done = t == STG_NONE;
+        }
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_u32(tile_id + s)), "r"(t) : "memory");
+        if (t == STG_NONE) {
+            mbar_arrive(&bar[s]);
+            return;
+        }
+        mbar_expect_tx(&bar[s], 2 * STG_TILE * EPP * 32);
+        uint8_t* dst = smem + s * STG_STAGE_BYTES;
+        const size_t y0 = (size_t)t * STG_TILE;
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(tp.in[jj]);
+            if (ORDER == ORDER_LOW_TO_HIGH) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) bulk_g2s(dst + jj * TOFF + q * (SUB + 16), src + (y0 + 32 * q) * EPP * 32, SUB, &bar[s]);
+            } else {
+#pragma unroll
+                for (int u = 0; u < EPP; ++u)
+                    bulk_g2s(dst + jj * TOFF + u * STG_TILE * 32, src + (y0 + u * pairs) * 32, STG_TILE * 32, &bar[s]);
+            }
+        }
+    };
+
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) mbar_init(&bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (tid == 0) {
+        // the tables were written through the generic proxy (by any block, last round); the bulk copies read them
+        // through the async proxy - after the command acquire, before the first copy
+        fence_proxy_async_global();
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) produce(s);
+    }
+    uint64_t* const out = j ? tp.out[1] : tp.out[0];
+    const uint32_t ring = smem_u32(smem);
+    uint32_t A[17];
+#pragma unroll
+    for (int w = 0; w < 17; ++w) A[w] = 0;
+    for (uint32_t it = 0;; ++it) {
+        const int s = (int)(it % STG_STAGES);
+        mbar_wait(&bar[s], (it / STG_STAGES) & 1);
+        uint32_t t;
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(t) : "r"(smem_u32(tile_id + s)));
+        if (t == STG_NONE) break;  // (block-uniform; the later stages hold no copy either: claims only run out once)
+        Fr e[EPP];
+#pragma unroll
+        for (int u = 0; u < EPP; ++u) e[u] = lds_fr(ring + s * STG_STAGE_BYTES + off + u * ESTEP);
+        __syncthreads();  // stage s is read out
+        if (tid == 0) produce(s);
+        const size_t y = (size_t)t * STG_TILE + p;
+        Fr lo, hi;
+        if (BIND) {
+            if (ORDER == ORDER_LOW_TO_HIGH) {
+                lo = bind_pair<HI4>(e[0], e[1], sc);
+                hi = bind_pair<HI4>(e[2], e[3], sc);
+                stg_fr(out, 2 * y, lo);
+                stg_fr(out, 2 * y + 1, hi);
+            } else {
+                lo = bind_pair<HI4>(e[0], e[2], sc);
+                hi = bind_pair<HI4>(e[1], e[3], sc);
+                stg_fr(out, y, lo);
+                stg_fr(out, y + pairs, hi);
+            }
+        } else {
+            lo = e[0];
+            hi = e[1];
+        }
+        const Fr dl = fp_sub_lazy(hi, lo);
+        Fr x, z;  // even thread: x = lo0, z = lo1; odd thread: x = dl0, z = dl1
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            const uint32_t got = __shfl_xor_sync(0xffffffffu, j ? lo.v[w] : dl.v[w], 1);
+            x.v[w] = j ? got : lo.v[w];
+            z.v[w] = j ? dl.v[w] : got;
+        }
+        mul_wide_acc_reg(A, x.v, z.v);
+    }
+    __syncthreads();  // every stage's last phase has been observed: no copy is in flight
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) mbar_inval(&bar[s]);
+    }
+    // column sums over the warp's even lanes (value 0) and odd lanes (value 1); 16-bit halves: no overflow in REDUX
+    uint64_t* red = reinterpret_cast<uint64_t*>(smem + STG_RED_OFF);
+#pragma unroll
+    for (int w = 0; w < 17; ++w) {
+        const uint32_t v0 = j ? 0u : A[w], v1 = j ? A[w] : 0u;
+        const uint64_t s0 = __reduce_add_sync(0xffffffffu, v0 & 0xffffu) + ((uint64_t)__reduce_add_sync(0xffffffffu, v0 >> 16) << 16);
+        const uint64_t s1 = __reduce_add_sync(0xffffffffu, v1 & 0xffffu) + ((uint64_t)__reduce_add_sync(0xffffffffu, v1 >> 16) << 16);
+        if (lane == 0) {
+            red[warp * 34 + w] = s0;
+            red[warp * 34 + 17 + w] = s1;
+        }
+    }
+    __syncthreads();
+    if (tid < 34) {
+        uint64_t v = 0;
+#pragma unroll
+        for (int wp = 0; wp < RES_BLOCK / 32; ++wp) v += red[wp * 34 + tid];
+        if (s_dst) s_dst[tid] = v;
+        else atomicAdd(reinterpret_cast<unsigned long long*>(g_lanes) + tid, (unsigned long long)v);
+    }
+}
+
 // lanes a member's round leaves in the accumulators / mailbox
 template <int D>
 __host__ __device__ constexpr int res_lanes(bool thin) {
@@ -351,7 +540,7 @@ template <int D, int P, int ORDER>
 __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __grid_constant__ ResArgs a) {
     constexpr int T = D * P;
     constexpr int K = D;  // s(1) always comes from the running claim (the optimized tier's convention)
-    extern __shared__ uint32_t dsm[];
+    extern __shared__ __align__(128) uint32_t dsm[];
     __shared__ uint64_t s_line[8];
     __shared__ uint64_t* s_cur[RES_MAX_MEMBERS][T];
     __shared__ uint64_t* s_oth[RES_MAX_MEMBERS][T];
@@ -558,16 +747,27 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                 }
                 tp.e_out = tp.e_in = nullptr;
                 tp.in_bits = 0;
+                tp.work = a.st->work + m * 32;
+                uint64_t* gl = a.st->lanes + m * RES_SLOT_U64;
+                uint64_t* sl = live == 1 ? s_lanes + m * RES_SLOT_U64 : nullptr;
+                if constexpr (D == 2 && P == 1) if (a.staged && sh.tpb == RES_BLOCK && pairs % STG_TILE == 0) {
+                    const uint32_t ntiles = (uint32_t)(pairs / STG_TILE);
+                    // passes of >= 2 tiles per block: the tail of the range is claimed tile by tile
+                    uint32_t static_end = ntiles;
+                    if (a.static_pct < 100 && live > 1 && ntiles >= 2 * sh.nblk)
+                        static_end = (uint32_t)((uint64_t)ntiles * (uint64_t)a.static_pct / 100 / sh.nblk * sh.nblk);
+                    const auto pass = !bind ? staged_pass<ORDER, false, false>
+                                      : hi4 ? staged_pass<ORDER, true, true> : staged_pass<ORDER, true, false>;
+                    pass(tp, pairs, sc(), reinterpret_cast<uint8_t*>(dsm), b, sh.nblk, static_end, gl, sl);
+                    continue;
+                }
                 // threads beyond this round's width have no pair (they still take part in the block reduction)
                 const size_t first = tid < (int)sh.tpb ? (size_t)b * sh.tpb + tid : (size_t)pairs;
                 const size_t stride = (size_t)sh.nblk * sh.tpb;
                 // passes of >= 2 full sweeps of the grid: the tail of the range is claimed warp by warp
-                tp.work = a.st->work + m * 32;
                 tp.static_end = ~(size_t)0;
                 if (a.static_pct < 100 && live > 1 && sh.tpb == RES_BLOCK && (size_t)pairs >= 2 * stride)
                     tp.static_end = ((size_t)pairs / 100 * (size_t)a.static_pct / stride) * stride;
-                uint64_t* gl = a.st->lanes + m * RES_SLOT_U64;
-                uint64_t* sl = live == 1 ? s_lanes + m * RES_SLOT_U64 : nullptr;
                 const auto pass = !bind ? resident_pass<D, P, ORDER, false, false>
                                   : hi4 ? resident_pass<D, P, ORDER, true, true> : resident_pass<D, P, ORDER, true, false>;
                 pass(tp, pairs, sc(), dsm, first, stride, gl, sl);
