@@ -169,6 +169,37 @@ int jb_member_final_evals(jb_member* mem, uint64_t* out_m_elems);
 int jb_eq_member_create(jb_ctx* ctx, const jb_table* tables, size_t m, const uint64_t* w, size_t nvars,
                         const uint64_t* scale_or_null, int order, jb_member** out);
 int jb_eq_member_scalar(jb_member* mem, uint64_t out[4]);
+/* Expression member: ProveRounds for any polynomial summand in up to 8 shared tables,
+ *   sum_x [eq(w, x) *] sum_k coeff_k * prod_{i < degree_k} f_{table_k[i]}(x),
+ * the relations of the reference tier's NaiveSumcheckProver (naive.rs:241-316) whose Expr is a weighted sum of
+ * monomials - Booleanity eq * (ra^2 - ra), the Spartan outer sumcheck eq * (Az Bz - Cz), read / write checking
+ * eq * (ra val + gamma wa val + gamma^2 wa inc). A table may appear in several monomials and several times in one; the
+ * monomials may differ in degree. Each round binds and reads every table once, whatever its multiplicity.
+ *  - Takes ownership of the ntables tables (distinct handles, one power-of-two length).
+ *  - degree D = the largest monomial degree, + 1 with an eq factor. With eq_w_or_null (nvars = log2(table length)
+ *    elements, w[0] <-> most significant index bit, optional scale) the eq factor is kept split as in
+ *    jb_eq_member_create: the running claim is mandatory in prove_round, a zero eq factor at the current variable is
+ *    refused, and jb_eq_member_scalar returns scale * eq(w, r) after the rounds.
+ *  - jb_member_final_evals returns the ntables bound values in table order (the output_claims inputs).
+ *  - A constant summand (a monomial of degree 0) is not supported: fold it into the claim.
+ * An expression that is exactly a built shape (unit coefficients, each table used once, monomials the consecutive
+ * blocks [kD, (k+1)D) of a product or sum of products, or with eq a single product of 1..3 tables) gets that member.
+ * Errors, before anything is allocated: JB_ERR_INVALID for a zero-degree monomial, a table index >= ntables, a table
+ * no monomial uses, duplicate handles, tables of different or non-power-of-two lengths, a non-canonical coefficient,
+ * point or scale, a scale without a point, nvars != log2(table length) with a point, an unknown order, no tables or no
+ * monomials; JB_ERR_UNSUPPORTED beyond the limits below. Expression members are not sharded
+ * (jb_member_prove_round_partials returns JB_ERR_UNSUPPORTED). */
+#define JB_EXPR_MAX_TABLES 8
+#define JB_EXPR_MAX_MONOMIALS 16
+#define JB_EXPR_MAX_DEGREE 6
+typedef struct jb_monomial {
+    uint64_t coeff[4];                      /* Montgomery limbs, canonical */
+    uint32_t degree;                        /* 1 .. JB_EXPR_MAX_DEGREE */
+    uint32_t table[JB_EXPR_MAX_DEGREE];     /* indices into `tables`, first `degree` used; repeats allowed (ra*ra) */
+} jb_monomial;
+int jb_member_create_expr(jb_ctx* ctx, const jb_table* tables, size_t ntables, const jb_monomial* monomials,
+                          size_t nmonomials, const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
+                          int order, jb_member** out);
 /* Multi-GPU: like prove_round but leaves this rank's partial sums - the kernel values s(0), [s(1) unless
  * skip_t1], s(2), .., s(m-1), s(inf) in the order jb_round_evals_from_kernel_values documents - on the device as
  * count x 8 uint64 lanes, each holding one 32-bit limb (exact under ncclSum over <= 2^32 ranks); the caller

@@ -18,6 +18,7 @@ from .api import (  # noqa: F401
     BatchMember,
     EqPolynomial,
     EqProductMember,
+    ExpressionMember,
     G1Bases,
     HyperKZG,
     HyperKZGProof,

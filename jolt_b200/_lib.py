@@ -56,6 +56,8 @@ SIGNATURES = {
     "jb_eq_member_create": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_u64p, c_size_t, c_u64p, ctypes.c_int,
                                            ctypes.POINTER(c_void_p)]),
     "jb_eq_member_scalar": (ctypes.c_int, [c_void_p, c_u64p]),
+    "jb_member_create_expr": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_void_p, c_size_t, c_u64p, c_size_t, c_u64p,
+                                             ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_prove_round_partials": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, c_void_p]),
     "jb_ctx_set_verify_rounds": (ctypes.c_int, [c_void_p, ctypes.c_int]),
     "jb_partials_finalize": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_u64p]),
@@ -122,6 +124,14 @@ class BatchMemberC(ctypes.Structure):
 class RoundWorkC(ctypes.Structure):
     _fields_ = [("member", c_size_t), ("round", c_size_t), ("has_bind", ctypes.c_int), ("has_claim", ctypes.c_int),
                 ("bind", ctypes.c_uint64 * 4), ("claim", ctypes.c_uint64 * 4)]
+
+
+JB_EXPR_MAX_TABLES, JB_EXPR_MAX_MONOMIALS, JB_EXPR_MAX_DEGREE = 8, 16, 6
+
+
+class MonomialC(ctypes.Structure):
+    _fields_ = [("coeff", ctypes.c_uint64 * 4), ("degree", ctypes.c_uint32),
+                ("table", ctypes.c_uint32 * JB_EXPR_MAX_DEGREE)]
 
 
 class FinishWorkC(ctypes.Structure):

@@ -491,6 +491,64 @@ class EqProductMember(ProductMember):
         return F.from_limbs(out)
 
 
+class ExpressionMember(ProductMember):
+    """ProveRounds member for any polynomial summand over shared tables (jb_member_create_expr):
+    sum_x [eq(w, x) *] sum_k c_k prod_i f_{tables_k[i]}(x) - the reference tier's NaiveSumcheckProver
+    (naive.rs:241-316) for an Expr that is a weighted sum of monomials. `monomials`: [(coefficient, [table indices])],
+    coefficient an int (taken mod r) or 4 Montgomery limbs; a table may repeat (ra * ra) and appear in several
+    monomials. With `w_limbs` (n elements, w[0] <-> MSB) the eq factor is kept split as in EqProductMember and the
+    running claim is mandatory. An expression that is exactly a built product / sum-of-products / eq-product shape is
+    served by that member. final_evals() returns every table's bound value in table order."""
+
+    def __init__(self, session: Session, polys: list[Polynomial], monomials, w_limbs=None, scale=None,
+                 order: int = HIGH_TO_LOW):
+        self.s = session
+        handles = np.array([p.handle for p in polys], dtype=np.uint64)
+        mons = (_lib.MonomialC * max(len(monomials), 1))()
+        for k, (coeff, tabs) in enumerate(monomials):
+            c = _limbs(coeff % F.R_MOD if isinstance(coeff, (int, np.integer)) else coeff)
+            mons[k].coeff[:] = [int(x) for x in c]
+            mons[k].degree = len(tabs)
+            for i, t in enumerate(list(tabs)[:_lib.JB_EXPR_MAX_DEGREE]):
+                mons[k].table[i] = int(t)
+        w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
+        sc = None if scale is None else _limbs(scale)
+        h = ctypes.c_void_p()
+        session.check(session.lib.jb_member_create_expr(
+            session.h, _p(handles), len(polys), ctypes.cast(mons, ctypes.c_void_p), len(monomials),
+            _p(w) if w is not None else None, 0 if w is None else w.shape[0], _p(sc) if sc is not None else None, order,
+            ctypes.byref(h)))
+        for p in polys:
+            p.handle = 0
+        self.h = h
+        self.ntables = len(polys)
+        d = ctypes.c_size_t()
+        session.check(session.lib.jb_member_degree(h, ctypes.byref(d)))
+        self._degree = d.value
+        self.m = d.value
+
+    def degree(self) -> int:
+        return self._degree
+
+    def prove_round_evals(self, bind, rnd: int, previous_claim=None) -> list[int]:
+        b = None if bind is None else _limbs(bind)
+        c = None if previous_claim is None else _limbs(previous_claim)
+        out = np.empty((self._degree + 1, 4), dtype=np.uint64)
+        self.s.check(self.s.lib.jb_member_prove_round(self.h, _p(b) if b is not None else None, rnd,
+                                                      _p(c) if c is not None else None, _p(out)))
+        return F.limbs_to_ints(out)
+
+    def final_evals(self, raw: bool = False):
+        out = np.empty((self.ntables, 4), dtype=np.uint64)
+        self.s.check(self.s.lib.jb_member_final_evals(self.h, _p(out)))
+        return out if raw else F.limbs_to_ints(out)
+
+    def eq_scalar(self) -> int:
+        out = np.empty(4, dtype=np.uint64)
+        self.s.check(self.s.lib.jb_eq_member_scalar(self.h, _p(out)))
+        return F.from_limbs(out)
+
+
 @dataclass
 class BatchMember:
     """jolt_sumcheck::BatchMember (batch.rs:24-71)."""

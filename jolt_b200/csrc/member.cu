@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -177,18 +178,70 @@ int dispatch_fused(jb_ctx* c, int m, int terms, int order, bool skip1, const Tab
     }
 }
 
+// expression members (expr_pass.cuh): EXPR_BLOCK threads per block, shared memory by the member's table count
+template <int ORDER, bool BIND, bool HI4, bool WEIGHTED>
+int launch_expr(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, const ExprParams& ex, RoundOut out) {
+    auto kernel = expr_round_kernel<ORDER, BIND, HI4, WEIGHTED>;
+    static const bool attr = [&] {
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)expr_smem_bytes(EXPR_MAX_TABLES));
+        return true;
+    }();
+    (void)attr;
+    static std::atomic<int> per_sm_by_tables[EXPR_MAX_TABLES + 1];  // occupancy depends on the shared memory size
+    const size_t smem = expr_smem_bytes(ex.ntables);
+    int per_sm = per_sm_by_tables[ex.ntables].load(std::memory_order_relaxed);
+    if (per_sm == 0) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, EXPR_BLOCK, smem) != cudaSuccess || per_sm < 1)
+            per_sm = 1;
+        per_sm_by_tables[ex.ntables].store(per_sm, std::memory_order_relaxed);
+    }
+    size_t need = (pairs + EXPR_BLOCK - 1) / EXPR_BLOCK;
+    size_t resident = (size_t)c->sm_count * per_sm;
+    size_t grid = need < resident ? need : resident;
+    if (grid < 1) grid = 1;
+    int st = c->ensure_partial(grid * EXPR_MAX_POINTS);
+    if (st != JB_OK) return st;
+    out.partial = c->d_partial;
+    int tix = c->timing_begin(BIND ? 0 : 2, pairs, ex.D);
+    const unsigned block = pairs <= 32 ? 32u : (unsigned)EXPR_BLOCK;
+    kernel<<<(unsigned)grid, block, smem, c->stream>>>(tp, pairs, s, ex, out);
+    c->timing_end(tix);
+    c->launches++;
+    return c->check(cudaGetLastError(), "expr_round_kernel launch");
+}
+
+template <int ORDER, bool WEIGHTED>
+int dispatch_expr2(jb_ctx* c, const TablePtrs& tp, size_t pairs, bool bind, bool hi4, const BindScalar& s,
+                   const ExprParams& ex, const RoundOut& out) {
+    if (!bind) return launch_expr<ORDER, false, false, WEIGHTED>(c, tp, pairs, s, ex, out);
+    return hi4 ? launch_expr<ORDER, true, true, WEIGHTED>(c, tp, pairs, s, ex, out)
+               : launch_expr<ORDER, true, false, WEIGHTED>(c, tp, pairs, s, ex, out);
+}
+
+// The round's evaluation points in kernel-value order: 0, [1 unless skip1], 2, .., D-1, inf (D >= 2); 0, [1] (D == 1).
+int dispatch_expr(jb_ctx* c, const jb_member* mem, bool weighted, bool skip1, const TablePtrs& tp, size_t pairs, bool bind,
+                  bool hi4, const BindScalar& s, const RoundOut& out) {
+    ExprParams ex = mem->ex;
+    int n = 0;
+    ex.point[n++] = 0;
+    if (!skip1) ex.point[n++] = 1;
+    for (int t = 2; t < ex.D; ++t) ex.point[n++] = (int8_t)t;
+    if (ex.D >= 2) ex.point[n++] = EXPR_INF;
+    ex.npoints = n;
+    if (mem->order == JB_LOW_TO_HIGH)
+        return weighted ? dispatch_expr2<ORDER_LOW_TO_HIGH, true>(c, tp, pairs, bind, hi4, s, ex, out)
+                        : dispatch_expr2<ORDER_LOW_TO_HIGH, false>(c, tp, pairs, bind, hi4, s, ex, out);
+    return weighted ? dispatch_expr2<ORDER_HIGH_TO_LOW, true>(c, tp, pairs, bind, hi4, s, ex, out)
+                    : dispatch_expr2<ORDER_HIGH_TO_LOW, false>(c, tp, pairs, bind, hi4, s, ex, out);
+}
+
 }  // namespace
 
 extern "C" {
 
 // ---- sumcheck member -------------------------------------------------------------------
-static int member_create_common(jb_ctx* c, const jb_table* handles, size_t m, size_t terms, int order, jb_member** out) {
-    if (!c || !handles || !out) return JB_ERR_INVALID;
-    Guard g(c);
-    if (!shape_supported((int)m, (int)terms))
-        return c->fail(JB_ERR_UNSUPPORTED, "member: supported shapes are products of 1..4 tables and 2 terms x 2 factors");
-    if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "member: unknown order");
-    const size_t T = m * terms;
+// The T handles name distinct tables of the context with one power-of-two length (context lock held).
+static int check_tables(jb_ctx* c, const jb_table* handles, size_t T, size_t* len_out) {
     size_t len = 0;
     for (size_t j = 0; j < T; ++j) {
         Table* t = c->find(handles[j]);
@@ -199,11 +252,18 @@ static int member_create_common(jb_ctx* c, const jb_table* handles, size_t m, si
         if (t->len != len) return c->fail(JB_ERR_INVALID, "member: tables differ in length");
     }
     if (len == 0 || (len & (len - 1))) return c->fail(JB_ERR_INVALID, "member: table length must be a power of two");
+    *len_out = len;
+    return JB_OK;
+}
+
+// A new member owning the T checked tables (context lock held).
+static int adopt_tables(jb_ctx* c, const jb_table* handles, size_t T, size_t len, int m, int terms, int order,
+                        jb_member** out) {
     jb_member* mem = new (std::nothrow) jb_member();
     if (!mem) return JB_ERR_OOM;
     mem->ctx = c;
-    mem->m = (int)m;
-    mem->terms = (int)terms;
+    mem->m = m;
+    mem->terms = terms;
     mem->order = order;
     mem->len = len;
     mem->rounds = 0;
@@ -215,6 +275,19 @@ static int member_create_common(jb_ctx* c, const jb_table* handles, size_t m, si
     }
     *out = mem;
     return JB_OK;
+}
+
+static int member_create_common(jb_ctx* c, const jb_table* handles, size_t m, size_t terms, int order, jb_member** out) {
+    if (!c || !handles || !out) return JB_ERR_INVALID;
+    Guard g(c);
+    if (!shape_supported((int)m, (int)terms))
+        return c->fail(JB_ERR_UNSUPPORTED, "member: supported shapes are products of 1..4 tables and 2 terms x 2 factors");
+    if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "member: unknown order");
+    const size_t T = m * terms;
+    size_t len = 0;
+    int st = check_tables(c, handles, T, &len);
+    if (st != JB_OK) return st;
+    return adopt_tables(c, handles, T, len, (int)m, (int)terms, order, out);
 }
 
 int jb_member_create(jb_ctx* c, const jb_table* handles, size_t m, int order, jb_member** out) {
@@ -318,9 +391,11 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
         tp.e_out = eqr->e_out;
         tp.e_in = eqr->e_in;
         tp.in_bits = eqr->in_bits;
-        st = dispatch_weighted(c, mem->m, mem->order, tp, pairs, do_bind, hi4, s, ro);
+        st = mem->expr ? dispatch_expr(c, mem, true, true, tp, pairs, do_bind, hi4, s, ro)
+                       : dispatch_weighted(c, mem->m, mem->order, tp, pairs, do_bind, hi4, s, ro);
     } else {
-        st = dispatch_fused(c, mem->m, mem->terms, mem->order, skip1, tp, pairs, do_bind, hi4, s, ro);
+        st = mem->expr ? dispatch_expr(c, mem, false, skip1, tp, pairs, do_bind, hi4, s, ro)
+                       : dispatch_fused(c, mem->m, mem->terms, mem->order, skip1, tp, pairs, do_bind, hi4, s, ro);
     }
     if (st != JB_OK) return st;
     if (do_bind) {
@@ -360,13 +435,15 @@ static int resident_values(int D, const uint64_t* lanes, uint64_t* vals);
 static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
 
 struct RoundConsts {
-    HostFr w[4], ipow[4], mpow;
+    HostFr w[6], ipow[6], mpow;
 };
-static const RoundConsts& round_consts(int M) {  // M in 2..4
-    static RoundConsts table[5];
+// M in 2..6: products of up to 4 tables; expression members up to degree 6 (jb_round_evals_from_kernel_values stays at 4)
+static const RoundConsts& round_consts(int M) {
+    static RoundConsts table[7];
     static const bool init = [] {
-        static const uint64_t binom[5][5] = {{1, 0, 0, 0, 0}, {1, 1, 0, 0, 0}, {1, 2, 1, 0, 0}, {1, 3, 3, 1, 0}, {1, 4, 6, 4, 1}};
-        for (int m = 2; m <= 4; ++m) {
+        static const uint64_t binom[7][7] = {{1}, {1, 1}, {1, 2, 1}, {1, 3, 3, 1}, {1, 4, 6, 4, 1}, {1, 5, 10, 10, 5, 1},
+                                             {1, 6, 15, 20, 15, 6, 1}};
+        for (int m = 2; m <= 6; ++m) {
             for (int i = 0; i < m; ++i) {
                 HostFr ti = HostFr::one();  // i^m
                 for (int e = 0; e < m; ++e) ti = ti * HostFr::from_u64((uint64_t)i);
@@ -688,22 +765,12 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     return JB_OK;
 }
 
-int jb_eq_member_create(jb_ctx* c, const jb_table* handles, size_t m, const uint64_t* w, size_t nvars,
-                        const uint64_t* scale_or_null, int order, jb_member** out) {
-    if (!c || !handles || !w || !out) return JB_ERR_INVALID;
-    if (order != JB_LOW_TO_HIGH && order != JB_HIGH_TO_LOW) return c->fail(JB_ERR_INVALID, "eq member: unknown binding order");
-    if (m < 1 || m > 3) return c->fail(JB_ERR_UNSUPPORTED, "eq member: m must be 1..3");
-    for (size_t i = 0; i < nvars; ++i)
-        if (!canonical_fr(w + 4 * i)) return c->fail(JB_ERR_INVALID, "eq member: point limbs not canonical");
-    if (scale_or_null && !canonical_fr(scale_or_null)) return c->fail(JB_ERR_INVALID, "eq member: scale not canonical");
-    int st = jb_member_create(c, handles, m, order, out);
-    if (st != JB_OK) return st;
-    jb_member* mem = *out;
-    if (mem->rounds != nvars || nvars == 0) {
-        jb_member_destroy(mem);
-        *out = nullptr;
-        return c->fail(JB_ERR_INVALID, "eq member: point length must equal log2(table length) >= 1");
-    }
+// Makes a new member split-eq weighted by eq(w, x) * scale: the host state and the prefix / suffix eq tables of its
+// order. w, nvars (== the member's rounds) and the scale have been checked. On failure the member is destroyed.
+static int eq_setup(jb_member* mem, const uint64_t* w, size_t nvars, const uint64_t* scale_or_null, jb_member** out) {
+    jb_ctx* c = mem->ctx;
+    const int order = mem->order;
+    int st = JB_OK;
     {
     Guard g(c);
     mem->eq = true;
@@ -750,6 +817,104 @@ int jb_eq_member_create(jb_ctx* c, const jb_table* handles, size_t m, const uint
         *out = nullptr;
     }
     return st;
+}
+
+int jb_eq_member_create(jb_ctx* c, const jb_table* handles, size_t m, const uint64_t* w, size_t nvars,
+                        const uint64_t* scale_or_null, int order, jb_member** out) {
+    if (!c || !handles || !w || !out) return JB_ERR_INVALID;
+    if (order != JB_LOW_TO_HIGH && order != JB_HIGH_TO_LOW) return c->fail(JB_ERR_INVALID, "eq member: unknown binding order");
+    if (m < 1 || m > 3) return c->fail(JB_ERR_UNSUPPORTED, "eq member: m must be 1..3");
+    for (size_t i = 0; i < nvars; ++i)
+        if (!canonical_fr(w + 4 * i)) return c->fail(JB_ERR_INVALID, "eq member: point limbs not canonical");
+    if (scale_or_null && !canonical_fr(scale_or_null)) return c->fail(JB_ERR_INVALID, "eq member: scale not canonical");
+    int st = jb_member_create(c, handles, m, order, out);
+    if (st != JB_OK) return st;
+    jb_member* mem = *out;
+    if (mem->rounds != nvars || nvars == 0) {
+        jb_member_destroy(mem);
+        *out = nullptr;
+        return c->fail(JB_ERR_INVALID, "eq member: point length must equal log2(table length) >= 1");
+    }
+    return eq_setup(mem, w, nvars, scale_or_null, out);
+}
+
+// ---- expression member ---------------------------------------------------------------------------------
+// Everything is checked before anything is allocated. An expression that is exactly a built shape - unit
+// coefficients, every table used once, monomials the consecutive blocks [kD, (k+1)D) of a product / sum of products
+// (no eq) or a single product of 1..3 tables (eq) - gets that member, so it keeps the resident kernel and the
+// specialised passes; anything else gets the expression pass.
+int jb_member_create_expr(jb_ctx* c, const jb_table* handles, size_t ntables, const jb_monomial* monomials,
+                          size_t nmonomials, const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
+                          int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    if (!handles || !monomials || !out) return JB_ERR_INVALID;
+    size_t len = 0;
+    int D = 0;
+    bool blocks = true;  // unit coefficients, every monomial of one degree, tables in consecutive blocks
+    bool own_pass = true;  // the expression pass serves it (else an existing member does)
+    {
+        Guard g(c);
+        if (ntables > JB_EXPR_MAX_TABLES || nmonomials > JB_EXPR_MAX_MONOMIALS)
+            return c->fail(JB_ERR_UNSUPPORTED, "expr member: at most JB_EXPR_MAX_TABLES tables and JB_EXPR_MAX_MONOMIALS monomials");
+        if (ntables == 0 || nmonomials == 0) return c->fail(JB_ERR_INVALID, "expr member: no tables or no monomials");
+        if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "expr member: unknown order");
+        const HostFr one = HostFr::one();
+        bool used[JB_EXPR_MAX_TABLES] = {false};
+        for (size_t k = 0; k < nmonomials; ++k) {
+            const jb_monomial& mo = monomials[k];
+            if (mo.degree == 0) return c->fail(JB_ERR_INVALID, "expr member: a monomial of degree 0 (constant summands are not supported)");
+            if (mo.degree > JB_EXPR_MAX_DEGREE) return c->fail(JB_ERR_UNSUPPORTED, "expr member: monomial degree above JB_EXPR_MAX_DEGREE");
+            if (!canonical_fr(mo.coeff)) return c->fail(JB_ERR_INVALID, "expr member: coefficient limbs not canonical");
+            for (uint32_t i = 0; i < mo.degree; ++i) {
+                if (mo.table[i] >= ntables) return c->fail(JB_ERR_INVALID, "expr member: table index out of range");
+                if (mo.table[i] != k * monomials[0].degree + i) blocks = false;
+                used[mo.table[i]] = true;
+            }
+            if (mo.degree != monomials[0].degree || HostFr::from_limbs(mo.coeff) != one) blocks = false;
+            D = std::max(D, (int)mo.degree);
+        }
+        for (size_t j = 0; j < ntables; ++j)
+            if (!used[j]) return c->fail(JB_ERR_INVALID, "expr member: a table no monomial uses");
+        if (ntables != nmonomials * monomials[0].degree) blocks = false;
+        if (eq_scale_or_null && !eq_w_or_null) return c->fail(JB_ERR_INVALID, "expr member: a scale without an eq point");
+        if (eq_w_or_null) {
+            for (size_t i = 0; i < nvars; ++i)
+                if (!canonical_fr(eq_w_or_null + 4 * i)) return c->fail(JB_ERR_INVALID, "expr member: point limbs not canonical");
+            if (eq_scale_or_null && !canonical_fr(eq_scale_or_null))
+                return c->fail(JB_ERR_INVALID, "expr member: scale not canonical");
+        }
+        int st = check_tables(c, handles, ntables, &len);
+        if (st != JB_OK) return st;
+        if (eq_w_or_null && (nvars == 0 || nvars >= 64 || ((size_t)1 << nvars) != len))
+            return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
+        own_pass = !blocks || (eq_w_or_null ? !(nmonomials == 1 && D <= 3) : !shape_supported(D, (int)nmonomials));
+        if (own_pass) {
+            st = adopt_tables(c, handles, ntables, len, D, 1, order, out);
+            if (st != JB_OK) return st;
+            jb_member* mem = *out;
+            mem->expr = true;
+            ExprParams& ex = mem->ex;
+            std::memset(&ex, 0, sizeof ex);
+            const HostFr minus_one = HostFr::zero() - one;
+            for (size_t k = 0; k < nmonomials; ++k) {
+                const jb_monomial& mo = monomials[k];
+                const HostFr cf = HostFr::from_limbs(mo.coeff);
+                for (int w = 0; w < 4; ++w) {
+                    ex.coeff[k][2 * w] = (uint32_t)mo.coeff[w];
+                    ex.coeff[k][2 * w + 1] = (uint32_t)(mo.coeff[w] >> 32);
+                }
+                for (uint32_t i = 0; i < mo.degree; ++i) ex.table[k][i] = (uint8_t)mo.table[i];
+                ex.degree[k] = (uint8_t)mo.degree;
+                ex.kind[k] = cf == one ? EXPR_COEFF_ONE : cf == minus_one ? EXPR_COEFF_MINUS_ONE : EXPR_COEFF_GENERAL;
+            }
+            ex.nmono = (int)nmonomials;
+            ex.ntables = (int)ntables;
+            ex.D = D;
+        }
+    }
+    if (own_pass) return eq_w_or_null ? eq_setup(*out, eq_w_or_null, nvars, eq_scale_or_null, out) : JB_OK;
+    if (eq_w_or_null) return jb_eq_member_create(c, handles, (size_t)D, eq_w_or_null, nvars, eq_scale_or_null, order, out);
+    return member_create_common(c, handles, (size_t)D, nmonomials, order, out);
 }
 
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
@@ -920,6 +1085,7 @@ int jb_member_prove_round_partials(jb_member* mem, const uint64_t* bind, size_t 
     (void)round;
     if (!mem || !lanes_out) return JB_ERR_INVALID;
     Guard g(mem->ctx, true);
+    if (mem->expr) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: expression members are not sharded");
     before_launch(mem);
     return member_round(mem, bind, skip_t1 != 0, lanes_out);
 }
@@ -1142,7 +1308,7 @@ int jb_scheduler_create(jb_ctx* c, jb_member** members, size_t n, jb_scheduler**
                 return c->fail(JB_ERR_INVALID, "scheduler: duplicate member");
             }
         s->members.push_back(m);
-        if (m->sharded || m->eq || m->m != members[0]->m || m->terms != members[0]->terms || m->order != members[0]->order)
+        if (m->sharded || m->eq || m->expr || members[0]->expr || m->m != members[0]->m || m->terms != members[0]->terms || m->order != members[0]->order)
             s->homogeneous = false;
     }
     *out = s;

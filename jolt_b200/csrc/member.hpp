@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "ctx.hpp"
+#include "expr_pass.cuh"
 #include "host_fr.hpp"
 #include "poly_kernels.cuh"
 #include "resident.cuh"
@@ -90,7 +91,11 @@ struct jb_member {
     bool look_ok = false;
     size_t look_round = 0;
     uint64_t look[6 * 4];
-    int ntables() const { return m * terms; }
+    // expression member (jb_member_create_expr): the summand is ex's weighted monomials over the tables (m = the
+    // largest monomial degree, `terms` unused); it never runs in a resident kernel
+    bool expr = false;
+    jb::ExprParams ex;
+    int ntables() const { return expr ? ex.ntables : m * terms; }
 };
 
 // resident.cu ------------------------------------------------------------------------------------------------
