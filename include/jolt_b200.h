@@ -378,6 +378,37 @@ int jb_msm_g1_table(jb_ctx* ctx, jb_srs bases, size_t offset, jb_table scalars, 
 int jb_msm_g1_one_hot_rows(jb_ctx* ctx, jb_srs bases, const void* const* columns, size_t count, int kind, size_t T,
                            size_t K, size_t row_width, int layout, uint64_t* out_xyz);
 
+/* ---- multilinear evaluation: Polynomial::evaluate (crates/jolt-poly/src/dense.rs:339-360) -------------------------
+ * value = sum_x f(x) eq(point, x), point[0] <-> the most significant index bit (as jb_eq_evals); coordinates are
+ * canonical Montgomery limbs (125-bit [0,0,lo,hi] challenges and full values alike). Equal to binding point[0],
+ * point[1], .. HighToLow, or the reversed point LowToHigh. One pass reads each entry once (32 B for a field entry) and
+ * never forms the eq table; results are exact and deterministic (integer lane sums). Errors are checked before anything
+ * is allocated: JB_ERR_INVALID for a null pointer, an unknown kind or layout, a length, T or K that is not a power of
+ * two, tables of different lengths, nvars != log2(length), non-canonical point limbs, and - found on the device, the
+ * context stays usable - a one-hot address >= K that is not the none value. JB_ERR_UNSUPPORTED beyond the limits:
+ * nvars <= 40; one-hot T < 2^31 and K <= 2^16. count == 0 -> JB_OK.
+ *
+ * Resident tables of length 2^nvars (bound ones included), which are not modified: out[i] = tables[i] at point. */
+int jb_table_evaluate_batch(jb_ctx* ctx, const jb_table* tables, size_t count, const uint64_t* point, size_t nvars,
+                            uint64_t* out);
+/* Compact columns (kinds[i] != JB_SCALAR_FR, may differ per column; len = 2^nvars entries each): the value of the
+ * promoted polynomial F::from(v) (negatives r - |v|, -0 is 0). on_device = 0: host arrays borrowed for the call (as
+ * jb_table_upload_small); 1: device pointers owned by the caller (e.g. torch tensors), read in place. */
+int jb_small_evaluate_batch(jb_ctx* ctx, const void* const* columns, size_t count, const int* kinds, size_t len,
+                            int on_device, const uint64_t* point, size_t nvars, uint64_t* out);
+/* One-hot polynomials: the 0/1 polynomial jb_msm_g1_one_hot_rows commits (same kinds, none value, layouts and flat
+ * index), from count address columns of T entries. point: log2(K T) coordinates; JB_ONE_HOT_CYCLE_MAJOR:
+ * r_cycle = point[0 .. log T), r_addr = the rest; JB_ONE_HOT_ADDRESS_MAJOR: r_addr first.
+ *   out[p] = sum_{j: addr_p[j] != none} eq(r_cycle, j) eq(r_addr, addr_p[j]). */
+int jb_one_hot_evaluate(jb_ctx* ctx, const void* const* columns, size_t count, int kind, size_t T, size_t K, int layout,
+                        int on_device, const uint64_t* point, uint64_t* out);
+/* The pushforward of eq(r_cycle, .) through each address column (r_cycle: log2 T coordinates): count NEW resident
+ * tables of K entries, G_p[k] = sum_{j: addr_p[j] = k} eq(r_cycle, j) - the cycle-major polynomial bound HighToLow by
+ * r_cycle, so sum_k eq(r_addr, k) G_p[k] is jb_one_hot_evaluate's value. Ordinary tables: they feed the product and
+ * expression members (the address phase of a one-hot read-checking sumcheck). Nothing is created on an error. */
+int jb_one_hot_pushforward(jb_ctx* ctx, const void* const* columns, size_t count, int kind, size_t T, size_t K,
+                           int on_device, const uint64_t* r_cycle, jb_table* out_tables);
+
 /* Batch affine addition: batch_g1_additions_multi_affine (crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150),
  * the one-hot / binary column path of Dory's tier-1 commitments (crates/jolt-dory/src/streaming.rs:68,128,152,201).
  * Set s is indices[set_offsets[s] .. set_offsets[s + 1]) into `bases`; out_xy receives one AFFINE point per set

@@ -30,9 +30,13 @@ from .api import (  # noqa: F401
     SumOfProductsMember,
     SumcheckError,
     UnivariatePoly,
+    evaluate_small,
     g1_affine_limbs,
     g1_jacobian_to_affine,
     msm,
+    one_hot_evaluate,
+    one_hot_pushforward,
+    point_limbs,
     prove_batch,
     prove_batch_native,
     small_scalars,

@@ -91,6 +91,13 @@ SIGNATURES = {
     "jb_msm_g1_one_hot_rows": (ctypes.c_int, [c_void_p, ctypes.c_uint64, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int,
                                               c_size_t, c_size_t, c_size_t, ctypes.c_int, c_u64p]),
     "jb_msm_g1_table": (ctypes.c_int, [c_void_p, ctypes.c_uint64, c_size_t, ctypes.c_uint64, c_size_t, c_u64p]),
+    "jb_table_evaluate_batch": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_u64p, c_size_t, c_u64p]),
+    "jb_small_evaluate_batch": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.POINTER(ctypes.c_int),
+                                               c_size_t, ctypes.c_int, c_u64p, c_size_t, c_u64p]),
+    "jb_one_hot_evaluate": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, c_size_t, c_size_t,
+                                           ctypes.c_int, ctypes.c_int, c_u64p, c_u64p]),
+    "jb_one_hot_pushforward": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, c_size_t,
+                                              c_size_t, ctypes.c_int, c_u64p, c_u64p]),
     "jb_ctx_diag": (ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_double)]),
     "jb_ctx_run_log": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.POINTER(c_size_t)]),
     "jb_ctx_timing_enable": (ctypes.c_int, [c_void_p, ctypes.c_int, ctypes.c_uint64]),

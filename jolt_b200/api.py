@@ -241,6 +241,156 @@ class Polynomial:
             self.s.check(self.s.lib.jb_table_free(self.s.h, self.handle))
             self.handle = 0
 
+    def evaluate(self, point) -> int:
+        """Polynomial::evaluate (dense.rs:339-360): sum_x f(x) eq(point, x), point[0] <-> the most significant index
+        bit. The table is left as it is (jb_table_evaluate_batch)."""
+        return Polynomial.batch_evaluate([self], point)[0]
+
+    @staticmethod
+    def batch_evaluate(polys: list["Polynomial"], point) -> list[int]:
+        """Every polynomial (one session, one length 2^len(point)) at the same point, in one pass per table."""
+        if not polys:
+            return []
+        s = polys[0].s
+        pt = point_limbs(point)
+        handles = np.array([p.handle for p in polys], dtype=np.uint64)
+        out = np.empty((len(polys), 4), dtype=np.uint64)
+        s.check(s.lib.jb_table_evaluate_batch(s.h, _p(handles), len(polys), _p(pt), pt.shape[0], _p(out)))
+        return F.limbs_to_ints(out)
+
+
+def point_limbs(point) -> np.ndarray:
+    """An evaluation point as (n, 4) Montgomery limbs: a uint64 array of shape (n, 4) is taken as limbs, anything else
+    as a sequence of canonical Python ints."""
+    if isinstance(point, np.ndarray) and point.dtype == np.uint64 and point.ndim == 2:
+        return np.ascontiguousarray(point)
+    vals = [int(v) for v in point]
+    return F.ints_to_limbs(vals) if vals else np.zeros((0, 4), dtype=np.uint64)
+
+
+def _is_device_tensor(x) -> bool:
+    return hasattr(x, "data_ptr") and getattr(x, "is_cuda", False)
+
+
+def _torch_kind(t) -> str | None:
+    import torch
+    names = {torch.uint8: "u8", torch.bool: "u8", torch.int64: "i64"}
+    for n, k in (("uint16", "u16"), ("uint32", "u32"), ("uint64", "u64")):
+        if hasattr(torch, n):
+            names[getattr(torch, n)] = k
+    return names.get(t.dtype)
+
+
+_KIND_BYTES = {"u8": 1, "u16": 2, "u32": 4, "u64": 8, "u128": 16, "i64": 8, "i128": 16, "s64": 16, "s128": 24}
+
+
+def evaluate_small(session: Session, columns, point, kinds=None) -> list[int]:
+    """Compact columns (Polynomial<T>, dense.rs:22-142) evaluated at `point` as the promoted polynomials F::from(v),
+    without promoting them (jb_small_evaluate_batch). `columns`: one column or a list of them, all of 2^len(point)
+    entries - numpy arrays / sequences as small_scalars takes them (host: borrowed for the call), or contiguous CUDA
+    torch tensors (read in place on the device; a 128-bit or sign-magnitude kind is named in `kinds` and the tensor holds
+    its raw records). `kinds`: None, one kind name for all, or one per column."""
+    if isinstance(columns, np.ndarray) and columns.ndim == 1 or _is_device_tensor(columns):
+        columns = [columns]
+    columns = list(columns)
+    if not columns:
+        return []
+    if kinds is None or isinstance(kinds, str):
+        kinds = [kinds] * len(columns)
+    if len(kinds) != len(columns):
+        raise ValueError("evaluate_small: one kind per column")
+    dev = [_is_device_tensor(c) for c in columns]
+    if any(dev) != all(dev):
+        raise ValueError("evaluate_small: columns must be all host arrays or all CUDA tensors")
+    keep, ptrs, ks, lens = [], [], [], []
+    for col, kind in zip(columns, kinds):
+        if dev[0]:
+            if not col.is_contiguous():
+                raise ValueError("evaluate_small: device columns must be contiguous")
+            kind = kind or _torch_kind(col)
+            if kind not in _KIND_BYTES:
+                raise ValueError(f"evaluate_small: unsupported device column dtype {col.dtype} (kind={kind})")
+            nbytes = col.numel() * col.element_size()
+            if nbytes % _KIND_BYTES[kind]:
+                raise ValueError("evaluate_small: tensor size is not a whole number of entries")
+            ptrs.append(col.data_ptr())
+            ks.append(SCALAR_KINDS[kind])
+            lens.append(nbytes // _KIND_BYTES[kind])
+        else:
+            a, k, n = small_scalars(col, kind)
+            keep.append(a)
+            ptrs.append(a.ctypes.data)
+            ks.append(k)
+            lens.append(n)
+    if len(set(lens)) != 1:
+        raise ValueError("evaluate_small: columns must have one length")
+    pt = point_limbs(point)
+    out = np.empty((len(columns), 4), dtype=np.uint64)
+    session.check(session.lib.jb_small_evaluate_batch(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs),
+                                                      (ctypes.c_int * len(ks))(*ks), lens[0], 1 if dev[0] else 0,
+                                                      _p(pt), pt.shape[0], _p(out)))
+    return F.limbs_to_ints(out)
+
+
+def _address_columns(columns, what: str):
+    """(pointers, kind, T, on_device, keep-alive) for one-hot address columns: uint8 / uint16 numpy arrays or CUDA
+    tensors (torch.uint8, torch.uint16, or torch.int16 read as raw 16-bit words), all of one dtype and length."""
+    if isinstance(columns, np.ndarray) and columns.ndim == 1 or _is_device_tensor(columns):
+        columns = [columns]
+    columns = list(columns)
+    if not columns:
+        return [], SCALAR_KINDS["u8"], 1, 0, []
+    if all(_is_device_tensor(c) for c in columns):
+        import torch
+        u16 = {torch.int16} | ({torch.uint16} if hasattr(torch, "uint16") else set())
+        dt = columns[0].dtype
+        if (dt != torch.uint8 and dt not in u16) or any(c.dtype != dt or c.dim() != 1 or not c.is_contiguous()
+                                                        or c.numel() != columns[0].numel() for c in columns):
+            raise ValueError(f"{what}: columns must be contiguous 1-D uint8 or 16-bit tensors of one dtype and length")
+        kind = SCALAR_KINDS["u8" if dt == torch.uint8 else "u16"]
+        return [c.data_ptr() for c in columns], kind, columns[0].numel(), 1, columns
+    cols = [np.ascontiguousarray(c) for c in columns]
+    dt = cols[0].dtype
+    if dt not in ONE_HOT_NONE or any(c.dtype != dt or c.ndim != 1 or c.shape != cols[0].shape for c in cols):
+        raise ValueError(f"{what}: columns must be 1-D uint8 or uint16 arrays of one dtype and length")
+    kind = SCALAR_KINDS["u8" if dt == np.uint8 else "u16"]
+    return [c.ctypes.data for c in cols], kind, cols[0].shape[0], 0, cols
+
+
+def one_hot_evaluate(session: Session, columns, K: int, point, layout: str = "cycle_major") -> list[int]:
+    """The one-hot (RA) polynomials of G1Bases.one_hot_rows - coefficient (k, j) = 1 iff column[j] == k, flat index
+    j K + k ("cycle_major") or k T + j ("address_major") - evaluated at `point` (log2(K T) coordinates) straight from
+    their address columns (jb_one_hot_evaluate): sum_j eq(r_cycle, j) eq(r_addr, addr_j) over the cycles that touched
+    an address. "cycle_major": r_cycle = point[:log T], r_addr = the rest; "address_major" the other way round."""
+    if layout not in ONE_HOT_LAYOUTS:
+        raise ValueError(f"one_hot_evaluate: layout must be one of {sorted(ONE_HOT_LAYOUTS)}")
+    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_evaluate")
+    if not ptrs:
+        return []
+    pt = point_limbs(point)
+    if K < 1 or T < 1 or pt.shape[0] != (K * T).bit_length() - 1:
+        raise ValueError("one_hot_evaluate: the point must have log2(K T) coordinates")
+    out = np.empty((len(ptrs), 4), dtype=np.uint64)
+    session.check(session.lib.jb_one_hot_evaluate(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs), kind, T, K,
+                                                  ONE_HOT_LAYOUTS[layout], dev, _p(pt), _p(out)))
+    return F.limbs_to_ints(out)
+
+
+def one_hot_pushforward(session: Session, columns, K: int, r_cycle) -> list[Polynomial]:
+    """G[k] = sum_{j: column[j] = k} eq(r_cycle, j) for each address column (jb_one_hot_pushforward): new device
+    polynomials of K entries - the cycle-major one-hot polynomial bound HighToLow by r_cycle (log2 T coordinates),
+    ready for the address phase of a read-checking sumcheck (ProductMember / ExpressionMember)."""
+    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_pushforward")
+    if not ptrs:
+        return []
+    pt = point_limbs(r_cycle)
+    if pt.shape[0] != T.bit_length() - 1:
+        raise ValueError("one_hot_pushforward: r_cycle must have log2(T) coordinates")
+    out = np.zeros(len(ptrs), dtype=np.uint64)
+    session.check(session.lib.jb_one_hot_pushforward(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs), kind,
+                                                     T, K, dev, _p(pt), _p(out)))
+    return [Polynomial(session, int(h)) for h in out]
+
 
 class EqPolynomial:
     """jolt_poly::EqPolynomial (eq.rs:24): tables in big-endian index order (r[0] <-> MSB)."""
