@@ -200,6 +200,44 @@ typedef struct jb_monomial {
 int jb_member_create_expr(jb_ctx* ctx, const jb_table* tables, size_t ntables, const jb_monomial* monomials,
                           size_t nmonomials, const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
                           int order, jb_member** out);
+/* Expression member over SOURCES: the relation of jb_member_create_expr, but a source may be a witness column in its
+ * own format instead of a field table - a compact integer column (Polynomial<T>) or a one-hot polynomial
+ * ra(r_addr, j) = eq(r_addr, addr[j]) given by its address column (the cycle phase of RA virtualization). The first
+ * two rounds read the columns as they are; round 1 binds them into field tables of len/2 entries, and from there on
+ * the member is an ordinary expression member. Round polynomials and final evaluations are bit-identical to
+ * jb_member_create_expr over the promoted (jb_table_upload_small) or gathered field tables.
+ *  - JB_SOURCE_TABLE: a field table of `len` entries; the member takes ownership, as jb_member_create_expr does.
+ *  - JB_SOURCE_COMPACT: `len` integers of `kind` (any jb_scalar_kind but JB_SCALAR_FR); value F::from(v).
+ *  - JB_SOURCE_ONE_HOT: `len` addresses of `kind` (JB_SCALAR_U8 / U16; the all-ones value is the none value, as in
+ *    jb_one_hot_evaluate); f(j) = eq(r_addr, addr[j]) with r_addr = log2 K canonical coordinates, r_addr[0] <-> the
+ *    address MSB, and 0 for the none value. K a power of two, 1 <= K <= 2^16.
+ * `values` and `r_addr` are borrowed for the call (on_device = 0: host memory; 1: caller-owned device memory): the
+ * columns are copied into member-owned device memory and each one-hot source's eq(r_addr, .) table (K entries) is built
+ * at creation, together with every buffer the member's rounds need, so JB_ERR_OOM can only arise here. The copies
+ * and eq tables are released when the sources are bound (round 1, or jb_member_finish_rounds when len = 2).
+ * jb_member_final_evals returns one value per source in source order: the compact column's promoted polynomial or
+ * ra(r_addr, r) at the challenge point r. Errors, before anything is allocated: those of jb_member_create_expr, plus
+ * JB_ERR_INVALID for an unknown source type or kind, K not a power of two or out of range, a non-canonical r_addr,
+ * len not a power of two >= 2, a table source of another length, on_device not 0 / 1, a misaligned device column,
+ * a null pointer; JB_ERR_UNSUPPORTED for more than JB_EXPR_MAX_TABLES sources or a one-hot len >= 2^31. An address
+ * >= K that is not the none value is found on the device during creation and returns JB_ERR_INVALID, with nothing
+ * left allocated and the table sources still the caller's. The member never runs in a resident kernel and is not
+ * sharded (jb_member_prove_round_partials returns JB_ERR_UNSUPPORTED). */
+#define JB_SOURCE_TABLE 0
+#define JB_SOURCE_COMPACT 1
+#define JB_SOURCE_ONE_HOT 2
+typedef struct jb_source {
+    int type;                 /* JB_SOURCE_* */
+    int kind;                 /* COMPACT / ONE_HOT: jb_scalar_kind of `values` */
+    int on_device;            /* COMPACT / ONE_HOT: 0 host memory, 1 caller-owned device memory */
+    jb_table table;           /* TABLE */
+    const void* values;       /* COMPACT / ONE_HOT: len entries */
+    size_t K;                 /* ONE_HOT */
+    const uint64_t* r_addr;   /* ONE_HOT: log2 K elements (may be NULL when K = 1) */
+} jb_source;
+int jb_member_create_expr_sources(jb_ctx* ctx, const jb_source* sources, size_t nsources, size_t len,
+                                  const jb_monomial* monomials, size_t nmonomials, const uint64_t* eq_w_or_null,
+                                  size_t nvars, const uint64_t* eq_scale_or_null, int order, jb_member** out);
 /* Multi-GPU: like prove_round but leaves this rank's partial sums - the kernel values s(0), [s(1) unless
  * skip_t1], s(2), .., s(m-1), s(inf) in the order jb_round_evals_from_kernel_values documents - on the device as
  * count x 8 uint64 lanes, each holding one 32-bit limb (exact under ncclSum over <= 2^32 ranks); the caller

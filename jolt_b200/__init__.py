@@ -15,6 +15,7 @@ from .api import (  # noqa: F401
     ONE_HOT_LAYOUTS,
     ONE_HOT_NONE,
     SCALAR_KINDS,
+    Source,
     BatchMember,
     EqPolynomial,
     EqProductMember,

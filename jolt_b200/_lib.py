@@ -58,6 +58,8 @@ SIGNATURES = {
     "jb_eq_member_scalar": (ctypes.c_int, [c_void_p, c_u64p]),
     "jb_member_create_expr": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_void_p, c_size_t, c_u64p, c_size_t, c_u64p,
                                              ctypes.c_int, ctypes.POINTER(c_void_p)]),
+    "jb_member_create_expr_sources": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_u64p,
+                                                     c_size_t, c_u64p, ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_prove_round_partials": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, c_void_p]),
     "jb_ctx_set_verify_rounds": (ctypes.c_int, [c_void_p, ctypes.c_int]),
     "jb_partials_finalize": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_u64p]),
@@ -139,6 +141,14 @@ JB_EXPR_MAX_TABLES, JB_EXPR_MAX_MONOMIALS, JB_EXPR_MAX_DEGREE = 8, 16, 6
 class MonomialC(ctypes.Structure):
     _fields_ = [("coeff", ctypes.c_uint64 * 4), ("degree", ctypes.c_uint32),
                 ("table", ctypes.c_uint32 * JB_EXPR_MAX_DEGREE)]
+
+
+JB_SOURCE_TABLE, JB_SOURCE_COMPACT, JB_SOURCE_ONE_HOT = 0, 1, 2
+
+
+class SourceC(ctypes.Structure):
+    _fields_ = [("type", ctypes.c_int), ("kind", ctypes.c_int), ("on_device", ctypes.c_int), ("table", ctypes.c_uint64),
+                ("values", c_void_p), ("K", c_size_t), ("r_addr", c_u64p)]
 
 
 class FinishWorkC(ctypes.Structure):

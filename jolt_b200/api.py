@@ -654,13 +654,7 @@ class ExpressionMember(ProductMember):
                  order: int = HIGH_TO_LOW):
         self.s = session
         handles = np.array([p.handle for p in polys], dtype=np.uint64)
-        mons = (_lib.MonomialC * max(len(monomials), 1))()
-        for k, (coeff, tabs) in enumerate(monomials):
-            c = _limbs(coeff % F.R_MOD if isinstance(coeff, (int, np.integer)) else coeff)
-            mons[k].coeff[:] = [int(x) for x in c]
-            mons[k].degree = len(tabs)
-            for i, t in enumerate(list(tabs)[:_lib.JB_EXPR_MAX_DEGREE]):
-                mons[k].table[i] = int(t)
+        mons = _monomials_c(monomials)
         w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
         sc = None if scale is None else _limbs(scale)
         h = ctypes.c_void_p()
@@ -697,6 +691,109 @@ class ExpressionMember(ProductMember):
         out = np.empty(4, dtype=np.uint64)
         self.s.check(self.s.lib.jb_eq_member_scalar(self.h, _p(out)))
         return F.from_limbs(out)
+
+    @classmethod
+    def from_sources(cls, session: Session, sources: list["Source"], monomials, w_limbs=None, scale=None,
+                     order: int = HIGH_TO_LOW) -> "ExpressionMember":
+        """The member of ExpressionMember over sources (jb_member_create_expr_sources): each table is a Source - a
+        device Polynomial, a compact integer column or a one-hot address column - and the columns are read as they
+        are until the member's second round binds them into field tables. Rounds and final_evals() (one value per
+        source, in order) are those of ExpressionMember over the promoted / gathered tables."""
+        lens = {s.length for s in sources}
+        if len(lens) != 1:
+            raise ValueError("from_sources: every source must have one length")
+        arr = (_lib.SourceC * max(len(sources), 1))()
+        keep = []
+        for i, src in enumerate(sources):
+            src._fill(arr[i], keep)
+        mons = _monomials_c(monomials)
+        w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
+        sc = None if scale is None else _limbs(scale)
+        h = ctypes.c_void_p()
+        session.check(session.lib.jb_member_create_expr_sources(
+            session.h, ctypes.cast(arr, ctypes.c_void_p), len(sources), lens.pop(), ctypes.cast(mons, ctypes.c_void_p),
+            len(monomials), _p(w) if w is not None else None, 0 if w is None else w.shape[0],
+            _p(sc) if sc is not None else None, order, ctypes.byref(h)))
+        for src in sources:
+            if src.poly is not None:
+                src.poly.handle = 0  # ownership moved into the member
+        self = cls.__new__(cls)
+        self.s = session
+        self.h = h
+        self.ntables = len(sources)
+        d = ctypes.c_size_t()
+        session.check(session.lib.jb_member_degree(h, ctypes.byref(d)))
+        self._degree = d.value
+        self.m = d.value
+        return self
+
+
+def _monomials_c(monomials):
+    mons = (_lib.MonomialC * max(len(monomials), 1))()
+    for k, (coeff, tabs) in enumerate(monomials):
+        c = _limbs(coeff % F.R_MOD if isinstance(coeff, (int, np.integer)) else coeff)
+        mons[k].coeff[:] = [int(x) for x in c]
+        mons[k].degree = len(tabs)
+        for i, t in enumerate(list(tabs)[:_lib.JB_EXPR_MAX_DEGREE]):
+            mons[k].table[i] = int(t)
+    return mons
+
+
+class Source:
+    """One table of ExpressionMember.from_sources. Build with Source.table / Source.compact / Source.one_hot; the
+    column is borrowed until the member is created (it is copied to the device then)."""
+
+    def __init__(self, type_: int, length: int, poly: Polynomial | None = None, ptr: int = 0, kind: int = 0,
+                 on_device: int = 0, K: int = 0, r_addr: np.ndarray | None = None, keep=None):
+        self.type, self.length, self.poly, self.ptr, self.kind = type_, length, poly, ptr, kind
+        self.on_device, self.K, self.r_addr, self.keep = on_device, K, r_addr, keep
+
+    @classmethod
+    def table(cls, poly: Polynomial) -> "Source":
+        """A device field polynomial; the member takes ownership of it."""
+        return cls(_lib.JB_SOURCE_TABLE, len(poly), poly=poly)
+
+    @classmethod
+    def compact(cls, values, kind: str | None = None) -> "Source":
+        """A compact integer column (Polynomial<T>) with value F::from(v): a numpy array or sequence as small_scalars
+        takes it, or a contiguous CUDA tensor (a 128-bit or sign-magnitude kind is named in `kind`, the tensor holding
+        its raw records)."""
+        if _is_device_tensor(values):
+            if not values.is_contiguous():
+                raise ValueError("Source.compact: device columns must be contiguous")
+            kind = kind or _torch_kind(values)
+            if kind not in _KIND_BYTES:
+                raise ValueError(f"Source.compact: unsupported device column dtype {values.dtype} (kind={kind})")
+            nbytes = values.numel() * values.element_size()
+            if nbytes % _KIND_BYTES[kind]:
+                raise ValueError("Source.compact: tensor size is not a whole number of entries")
+            return cls(_lib.JB_SOURCE_COMPACT, nbytes // _KIND_BYTES[kind], ptr=values.data_ptr(),
+                       kind=SCALAR_KINDS[kind], on_device=1, keep=values)
+        a, k, n = small_scalars(values, kind)
+        return cls(_lib.JB_SOURCE_COMPACT, n, ptr=a.ctypes.data, kind=k, keep=a)
+
+    @classmethod
+    def one_hot(cls, addresses, K: int, r_addr) -> "Source":
+        """The one-hot polynomial ra(r_addr, j) = eq(r_addr, addresses[j]) (0 where the column holds the none value,
+        the all-ones value of its width): a uint8 / uint16 numpy array or CUDA tensor, K a power of two, r_addr
+        log2 K coordinates (r_addr[0] <-> the address MSB)."""
+        ptrs, kind, T, dev, keep = _address_columns(addresses, "Source.one_hot")
+        if len(ptrs) != 1:
+            raise ValueError("Source.one_hot: one address column")
+        r = point_limbs(r_addr)
+        if K < 1 or r.shape[0] != K.bit_length() - 1:
+            raise ValueError("Source.one_hot: r_addr must have log2(K) coordinates")
+        return cls(_lib.JB_SOURCE_ONE_HOT, T, ptr=ptrs[0], kind=kind, on_device=dev, K=K, r_addr=r, keep=keep)
+
+    def _fill(self, c, keep: list):
+        c.type, c.kind, c.on_device = self.type, self.kind, self.on_device
+        if self.poly is not None:
+            c.table = self.poly.handle
+        c.values = self.ptr or None
+        c.K = self.K
+        if self.r_addr is not None and self.r_addr.shape[0]:
+            c.r_addr = _p(self.r_addr)
+        keep.append(self)
 
 
 @dataclass

@@ -21,20 +21,12 @@ namespace {
 
 using Guard = CtxGuard;
 
-__device__ __forceinline__ Fr promote(const uint32_t mag[4], bool neg) {
-    Fr k = Fr::zero();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) k.v[j] = mag[j];
-    Fr m = fp_to_mont(k);  // |v| < 2^128 < r: already canonical as an integer
-    return neg ? fp_neg(m) : m;
-}
-
 __global__ void __launch_bounds__(256) promote_small_kernel(const void* values, size_t n, int kind, uint64_t* out) {
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         uint32_t mag[4];
         const bool neg = ld_small(values, i, kind, mag);
-        st_elem(out, i, promote(mag, neg));
+        st_elem(out, i, promote_small(mag, neg));
     }
 }
 
@@ -73,7 +65,7 @@ __global__ void __launch_bounds__(256) bind_small_kernel(const void* values, siz
         }
         Fr t = fp_mul(D, sv);  // s * |d| (Montgomery form)
         if (nd) t = fp_neg(t);
-        st_elem(out, i, fp_add(promote(ml, nl), t));
+        st_elem(out, i, fp_add(promote_small(ml, nl), t));
     }
 }
 

@@ -48,6 +48,48 @@ __device__ __forceinline__ void expr_st(uint32_t* col, int word0, const Fr& x) {
     for (int w = 0; w < 8; ++w) col[(word0 + w) * EXPR_BLOCK] = x.v[w];
 }
 
+// Steps 2 and 3 of a pair y whose bound (lo_j, D_j) are in the thread's columns: the monomials at every point of
+// the round, times the split-eq weight (WEIGHTED), added to acc. Shared by every pass that stages pairs this way.
+template <bool WEIGHTED>
+__device__ __forceinline__ void expr_sweep(uint32_t* col, const ExprParams& ex, const TablePtrs& tp, size_t y,
+                                           Fr (&acc)[EXPR_MAX_POINTS]) {
+    Fr wgt;
+    if (WEIGHTED) {  // the split-eq weight of the pair, formed where it is used
+        const size_t yo = y >> tp.in_bits;
+        wgt = fp_mul(ld_elem<Fr>(tp.e_out, yo), ld_elem<Fr>(tp.e_in, y - (yo << tp.in_bits)));
+    }
+    int at = 0;  // the point the value words of the columns hold
+#pragma unroll
+    for (int e = 0; e < EXPR_MAX_POINTS; ++e) {
+        if (e >= ex.npoints) break;
+        const int t = ex.point[e];
+        const bool inf = t == EXPR_INF;
+        for (; !inf && at < t; ++at)
+            for (int j = 0; j < ex.ntables; ++j) expr_st(col, 16 * j, fp_add(expr_ld(col, 16 * j), expr_ld(col, 16 * j + 8)));
+        const int off = inf ? 8 : 0;
+        Fr sum = Fr::zero();
+        for (int k = 0; k < ex.nmono; ++k) {
+            const int d = ex.degree[k];
+            if (inf && d < ex.D) continue;
+            Fr prod = expr_ld(col, 16 * ex.table[k][0] + off);
+            for (int i = 1; i < d; ++i) prod = fp_mul(prod, expr_ld(col, 16 * ex.table[k][i] + off));
+            const int kind = ex.kind[k];
+            if (kind == EXPR_COEFF_ONE) {
+                sum = fp_add(sum, prod);
+            } else if (kind == EXPR_COEFF_MINUS_ONE) {
+                sum = fp_sub(sum, prod);
+            } else {
+                Fr c;
+#pragma unroll
+                for (int w = 0; w < 8; ++w) c.v[w] = ex.coeff[k][w];
+                sum = fp_add(sum, fp_mul(prod, c));
+            }
+        }
+        if (WEIGHTED) sum = fp_mul(sum, wgt);
+        acc[e] = fp_add(acc[e], sum);
+    }
+}
+
 // One launch per round, one thread per pair index y (grid-stride). Binding and the table layouts are those of
 // fused_pass (HighToLow in place, LowToHigh ping-pong; BIND / HI4 / the 125-bit challenge path). Per pair:
 //   1. every table is bound once (BIND) or read, and (lo_j, D_j = hi_j - lo_j) goes to the thread's column;
@@ -110,41 +152,7 @@ __global__ void __launch_bounds__(EXPR_BLOCK, 4) expr_round_kernel(const __grid_
             expr_st(col, 16 * j, lo);
             expr_st(col, 16 * j + 8, fp_sub(hi, lo));
         }
-        Fr wgt;
-        if (WEIGHTED) {  // the split-eq weight of the pair, formed where it is used
-            const size_t yo = y >> tp.in_bits;
-            wgt = fp_mul(ld_elem<Fr>(tp.e_out, yo), ld_elem<Fr>(tp.e_in, y - (yo << tp.in_bits)));
-        }
-        int at = 0;  // the point the value words of the columns hold
-#pragma unroll
-        for (int e = 0; e < EXPR_MAX_POINTS; ++e) {
-            if (e >= ex.npoints) break;
-            const int t = ex.point[e];
-            const bool inf = t == EXPR_INF;
-            for (; !inf && at < t; ++at)
-                for (int j = 0; j < ex.ntables; ++j) expr_st(col, 16 * j, fp_add(expr_ld(col, 16 * j), expr_ld(col, 16 * j + 8)));
-            const int off = inf ? 8 : 0;
-            Fr sum = Fr::zero();
-            for (int k = 0; k < ex.nmono; ++k) {
-                const int d = ex.degree[k];
-                if (inf && d < ex.D) continue;
-                Fr prod = expr_ld(col, 16 * ex.table[k][0] + off);
-                for (int i = 1; i < d; ++i) prod = fp_mul(prod, expr_ld(col, 16 * ex.table[k][i] + off));
-                const int kind = ex.kind[k];
-                if (kind == EXPR_COEFF_ONE) {
-                    sum = fp_add(sum, prod);
-                } else if (kind == EXPR_COEFF_MINUS_ONE) {
-                    sum = fp_sub(sum, prod);
-                } else {
-                    Fr c;
-#pragma unroll
-                    for (int w = 0; w < 8; ++w) c.v[w] = ex.coeff[k][w];
-                    sum = fp_add(sum, fp_mul(prod, c));
-                }
-            }
-            if (WEIGHTED) sum = fp_mul(sum, wgt);
-            acc[e] = fp_add(acc[e], sum);
-        }
+        expr_sweep<WEIGHTED>(col, ex, tp, y, acc);
     }
     block_sum<EXPR_MAX_POINTS>(acc, red);
     round_epilogue<EXPR_MAX_POINTS>(acc, red, out);

@@ -16,6 +16,7 @@
 
 #include "member.hpp"
 #include "resident.cuh"
+#include "small_scalar.cuh"
 #include "sumcheck_host.hpp"
 #include "tma_ab.cuh"
 
@@ -228,6 +229,7 @@ int dispatch_expr(jb_ctx* c, const jb_member* mem, bool weighted, bool skip1, co
     for (int t = 2; t < ex.D; ++t) ex.point[n++] = (int8_t)t;
     if (ex.D >= 2) ex.point[n++] = EXPR_INF;
     ex.npoints = n;
+    if (!mem->src.empty()) return sources_round(c, mem, weighted, tp, pairs, bind, s, ex, out);  // rounds 0 and 1
     if (mem->order == JB_LOW_TO_HIGH)
         return weighted ? dispatch_expr2<ORDER_LOW_TO_HIGH, true>(c, tp, pairs, bind, hi4, s, ex, out)
                         : dispatch_expr2<ORDER_LOW_TO_HIGH, false>(c, tp, pairs, bind, hi4, s, ex, out);
@@ -348,10 +350,16 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
     TablePtrs tp;
     std::memset(&tp, 0, sizeof tp);
     const int T = mem->ntables();
+    const bool from_src = !mem->src.empty();
+    auto is_src = [&](int j) { return from_src && mem->src[j].type != JB_SOURCE_TABLE; };
     for (int j = 0; j < T; ++j) {
         Table& t = mem->tables[j];
         tp.in[j] = t.buf;
         tp.out[j] = t.buf;
+        if (is_src(j)) {  // read from its column; the bind writes the len/2 buffer allocated at creation
+            tp.in[j] = nullptr;
+            continue;
+        }
         if (do_bind && mem->order == JB_LOW_TO_HIGH) {
             int st = c->ensure_alt(t, len);
             if (st != JB_OK) return st;
@@ -400,10 +408,11 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
     if (st != JB_OK) return st;
     if (do_bind) {
         for (int j = 0; j < T; ++j) {
-            if (mem->order == JB_LOW_TO_HIGH) mem->tables[j].swap_buffers();
+            if (mem->order == JB_LOW_TO_HIGH && !is_src(j)) mem->tables[j].swap_buffers();
             mem->tables[j].len = len;
         }
         mem->len = len;
+        if (from_src) sources_release(mem);  // (stream-ordered: the columns are freed after the pass has read them)
     }
     return JB_OK;
 }
@@ -839,6 +848,69 @@ int jb_eq_member_create(jb_ctx* c, const jb_table* handles, size_t m, const uint
 }
 
 // ---- expression member ---------------------------------------------------------------------------------
+// The checks on the expression shared by both constructors (context lock held): D = the largest monomial degree;
+// blocks = unit coefficients, every monomial of one degree, tables in consecutive blocks.
+static int check_expr(jb_ctx* c, size_t ntables, const jb_monomial* monomials, size_t nmonomials,
+                      const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null, int order, int* D_out,
+                      bool* blocks_out) {
+    int D = 0;
+    bool blocks = true;
+    if (ntables > JB_EXPR_MAX_TABLES || nmonomials > JB_EXPR_MAX_MONOMIALS)
+        return c->fail(JB_ERR_UNSUPPORTED, "expr member: at most JB_EXPR_MAX_TABLES tables and JB_EXPR_MAX_MONOMIALS monomials");
+    if (ntables == 0 || nmonomials == 0) return c->fail(JB_ERR_INVALID, "expr member: no tables or no monomials");
+    if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "expr member: unknown order");
+    const HostFr one = HostFr::one();
+    bool used[JB_EXPR_MAX_TABLES] = {false};
+    for (size_t k = 0; k < nmonomials; ++k) {
+        const jb_monomial& mo = monomials[k];
+        if (mo.degree == 0) return c->fail(JB_ERR_INVALID, "expr member: a monomial of degree 0 (constant summands are not supported)");
+        if (mo.degree > JB_EXPR_MAX_DEGREE) return c->fail(JB_ERR_UNSUPPORTED, "expr member: monomial degree above JB_EXPR_MAX_DEGREE");
+        if (!canonical_fr(mo.coeff)) return c->fail(JB_ERR_INVALID, "expr member: coefficient limbs not canonical");
+        for (uint32_t i = 0; i < mo.degree; ++i) {
+            if (mo.table[i] >= ntables) return c->fail(JB_ERR_INVALID, "expr member: table index out of range");
+            if (mo.table[i] != k * monomials[0].degree + i) blocks = false;
+            used[mo.table[i]] = true;
+        }
+        if (mo.degree != monomials[0].degree || HostFr::from_limbs(mo.coeff) != one) blocks = false;
+        D = std::max(D, (int)mo.degree);
+    }
+    for (size_t j = 0; j < ntables; ++j)
+        if (!used[j]) return c->fail(JB_ERR_INVALID, "expr member: a table no monomial uses");
+    if (ntables != nmonomials * monomials[0].degree) blocks = false;
+    if (eq_scale_or_null && !eq_w_or_null) return c->fail(JB_ERR_INVALID, "expr member: a scale without an eq point");
+    if (eq_w_or_null) {
+        for (size_t i = 0; i < nvars; ++i)
+            if (!canonical_fr(eq_w_or_null + 4 * i)) return c->fail(JB_ERR_INVALID, "expr member: point limbs not canonical");
+        if (eq_scale_or_null && !canonical_fr(eq_scale_or_null))
+            return c->fail(JB_ERR_INVALID, "expr member: scale not canonical");
+    }
+    *D_out = D;
+    *blocks_out = blocks;
+    return JB_OK;
+}
+
+// Makes `mem` an expression member: the kernel parameter form of the checked monomials.
+static void make_expr(jb_member* mem, const jb_monomial* monomials, size_t nmonomials, size_t ntables, int D) {
+    mem->expr = true;
+    ExprParams& ex = mem->ex;
+    std::memset(&ex, 0, sizeof ex);
+    const HostFr one = HostFr::one(), minus_one = HostFr::zero() - one;
+    for (size_t k = 0; k < nmonomials; ++k) {
+        const jb_monomial& mo = monomials[k];
+        const HostFr cf = HostFr::from_limbs(mo.coeff);
+        for (int w = 0; w < 4; ++w) {
+            ex.coeff[k][2 * w] = (uint32_t)mo.coeff[w];
+            ex.coeff[k][2 * w + 1] = (uint32_t)(mo.coeff[w] >> 32);
+        }
+        for (uint32_t i = 0; i < mo.degree; ++i) ex.table[k][i] = (uint8_t)mo.table[i];
+        ex.degree[k] = (uint8_t)mo.degree;
+        ex.kind[k] = cf == one ? EXPR_COEFF_ONE : cf == minus_one ? EXPR_COEFF_MINUS_ONE : EXPR_COEFF_GENERAL;
+    }
+    ex.nmono = (int)nmonomials;
+    ex.ntables = (int)ntables;
+    ex.D = D;
+}
+
 // Everything is checked before anything is allocated. An expression that is exactly a built shape - unit
 // coefficients, every table used once, monomials the consecutive blocks [kD, (k+1)D) of a product / sum of products
 // (no eq) or a single product of 1..3 tables (eq) - gets that member, so it keeps the resident kernel and the
@@ -854,36 +926,9 @@ int jb_member_create_expr(jb_ctx* c, const jb_table* handles, size_t ntables, co
     bool own_pass = true;  // the expression pass serves it (else an existing member does)
     {
         Guard g(c);
-        if (ntables > JB_EXPR_MAX_TABLES || nmonomials > JB_EXPR_MAX_MONOMIALS)
-            return c->fail(JB_ERR_UNSUPPORTED, "expr member: at most JB_EXPR_MAX_TABLES tables and JB_EXPR_MAX_MONOMIALS monomials");
-        if (ntables == 0 || nmonomials == 0) return c->fail(JB_ERR_INVALID, "expr member: no tables or no monomials");
-        if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "expr member: unknown order");
-        const HostFr one = HostFr::one();
-        bool used[JB_EXPR_MAX_TABLES] = {false};
-        for (size_t k = 0; k < nmonomials; ++k) {
-            const jb_monomial& mo = monomials[k];
-            if (mo.degree == 0) return c->fail(JB_ERR_INVALID, "expr member: a monomial of degree 0 (constant summands are not supported)");
-            if (mo.degree > JB_EXPR_MAX_DEGREE) return c->fail(JB_ERR_UNSUPPORTED, "expr member: monomial degree above JB_EXPR_MAX_DEGREE");
-            if (!canonical_fr(mo.coeff)) return c->fail(JB_ERR_INVALID, "expr member: coefficient limbs not canonical");
-            for (uint32_t i = 0; i < mo.degree; ++i) {
-                if (mo.table[i] >= ntables) return c->fail(JB_ERR_INVALID, "expr member: table index out of range");
-                if (mo.table[i] != k * monomials[0].degree + i) blocks = false;
-                used[mo.table[i]] = true;
-            }
-            if (mo.degree != monomials[0].degree || HostFr::from_limbs(mo.coeff) != one) blocks = false;
-            D = std::max(D, (int)mo.degree);
-        }
-        for (size_t j = 0; j < ntables; ++j)
-            if (!used[j]) return c->fail(JB_ERR_INVALID, "expr member: a table no monomial uses");
-        if (ntables != nmonomials * monomials[0].degree) blocks = false;
-        if (eq_scale_or_null && !eq_w_or_null) return c->fail(JB_ERR_INVALID, "expr member: a scale without an eq point");
-        if (eq_w_or_null) {
-            for (size_t i = 0; i < nvars; ++i)
-                if (!canonical_fr(eq_w_or_null + 4 * i)) return c->fail(JB_ERR_INVALID, "expr member: point limbs not canonical");
-            if (eq_scale_or_null && !canonical_fr(eq_scale_or_null))
-                return c->fail(JB_ERR_INVALID, "expr member: scale not canonical");
-        }
-        int st = check_tables(c, handles, ntables, &len);
+        int st = check_expr(c, ntables, monomials, nmonomials, eq_w_or_null, nvars, eq_scale_or_null, order, &D, &blocks);
+        if (st != JB_OK) return st;
+        st = check_tables(c, handles, ntables, &len);
         if (st != JB_OK) return st;
         if (eq_w_or_null && (nvars == 0 || nvars >= 64 || ((size_t)1 << nvars) != len))
             return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
@@ -891,30 +936,131 @@ int jb_member_create_expr(jb_ctx* c, const jb_table* handles, size_t ntables, co
         if (own_pass) {
             st = adopt_tables(c, handles, ntables, len, D, 1, order, out);
             if (st != JB_OK) return st;
-            jb_member* mem = *out;
-            mem->expr = true;
-            ExprParams& ex = mem->ex;
-            std::memset(&ex, 0, sizeof ex);
-            const HostFr minus_one = HostFr::zero() - one;
-            for (size_t k = 0; k < nmonomials; ++k) {
-                const jb_monomial& mo = monomials[k];
-                const HostFr cf = HostFr::from_limbs(mo.coeff);
-                for (int w = 0; w < 4; ++w) {
-                    ex.coeff[k][2 * w] = (uint32_t)mo.coeff[w];
-                    ex.coeff[k][2 * w + 1] = (uint32_t)(mo.coeff[w] >> 32);
-                }
-                for (uint32_t i = 0; i < mo.degree; ++i) ex.table[k][i] = (uint8_t)mo.table[i];
-                ex.degree[k] = (uint8_t)mo.degree;
-                ex.kind[k] = cf == one ? EXPR_COEFF_ONE : cf == minus_one ? EXPR_COEFF_MINUS_ONE : EXPR_COEFF_GENERAL;
-            }
-            ex.nmono = (int)nmonomials;
-            ex.ntables = (int)ntables;
-            ex.D = D;
+            make_expr(*out, monomials, nmonomials, ntables, D);
         }
     }
     if (own_pass) return eq_w_or_null ? eq_setup(*out, eq_w_or_null, nvars, eq_scale_or_null, out) : JB_OK;
     if (eq_w_or_null) return jb_eq_member_create(c, handles, (size_t)D, eq_w_or_null, nvars, eq_scale_or_null, order, out);
     return member_create_common(c, handles, (size_t)D, nmonomials, order, out);
+}
+
+// ---- expression member over sources ---------------------------------------------------------------------
+// The checks on one source (context lock held). log_k: log2 K of a one-hot source.
+static int check_source(jb_ctx* c, const jb_source& sr, size_t len, size_t* log_k) {
+    if (sr.type == JB_SOURCE_TABLE) {
+        const Table* t = c->find(sr.table);
+        if (!t) return c->fail(JB_ERR_INVALID, "expr sources: unknown table handle");
+        if (t->len != len) return c->fail(JB_ERR_INVALID, "expr sources: a table source of another length");
+        return JB_OK;
+    }
+    if (sr.type != JB_SOURCE_COMPACT && sr.type != JB_SOURCE_ONE_HOT)
+        return c->fail(JB_ERR_INVALID, "expr sources: unknown source type");
+    const bool one_hot = sr.type == JB_SOURCE_ONE_HOT;
+    if (one_hot ? (sr.kind != JB_SCALAR_U8 && sr.kind != JB_SCALAR_U16) : (sr.kind < JB_SCALAR_U8 || sr.kind > JB_SCALAR_S128))
+        return c->fail(JB_ERR_INVALID, "expr sources: unknown kind (one-hot: JB_SCALAR_U8 / U16; compact: not JB_SCALAR_FR)");
+    if (!sr.values) return c->fail(JB_ERR_INVALID, "expr sources: null column");
+    if (sr.on_device != 0 && sr.on_device != 1) return c->fail(JB_ERR_INVALID, "expr sources: on_device must be 0 or 1");
+    const size_t align = std::min(8, small_kind_bytes(sr.kind));
+    if (sr.on_device && (uintptr_t)sr.values % align) return c->fail(JB_ERR_INVALID, "expr sources: misaligned device column");
+    if (!one_hot) return JB_OK;
+    if (sr.K == 0 || (sr.K & (sr.K - 1)) || sr.K > ((size_t)1 << 16))
+        return c->fail(JB_ERR_INVALID, "expr sources: K must be a power of two in [1, 2^16]");
+    if (len >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "expr sources: a one-hot column must be shorter than 2^31");
+    *log_k = 0;
+    while (((size_t)1 << *log_k) < sr.K) ++*log_k;
+    if (*log_k && !sr.r_addr) return c->fail(JB_ERR_INVALID, "expr sources: null r_addr");
+    for (size_t i = 0; i < *log_k; ++i)
+        if (!canonical_fr(sr.r_addr + 4 * i)) return c->fail(JB_ERR_INVALID, "expr sources: r_addr limbs not canonical");
+    return JB_OK;
+}
+
+// Frees what a failed creation had allocated (context lock held; the table sources were not adopted yet).
+static void discard_sources(jb_member* mem) {
+    sources_release(mem);
+    for (auto& t : mem->tables) mem->ctx->release(t);
+    delete mem;
+}
+
+int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
+                                  const jb_monomial* monomials, size_t nmonomials, const uint64_t* eq_w_or_null,
+                                  size_t nvars, const uint64_t* eq_scale_or_null, int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    if (!sources || !monomials || !out) return c->fail(JB_ERR_INVALID, "expr sources: null pointer");
+    jb_member* mem = nullptr;
+    int st = JB_OK;
+    {
+        Guard g(c);
+        int D = 0;
+        bool blocks = false;
+        st = check_expr(c, nsources, monomials, nmonomials, eq_w_or_null, nvars, eq_scale_or_null, order, &D, &blocks);
+        if (st != JB_OK) return st;
+        if (len < 2 || (len & (len - 1))) return c->fail(JB_ERR_INVALID, "expr sources: len must be a power of two >= 2");
+        if (eq_w_or_null && (nvars >= 64 || ((size_t)1 << nvars) != len))
+            return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
+        size_t log_k[JB_EXPR_MAX_TABLES] = {0};
+        for (size_t i = 0; i < nsources; ++i) {
+            if ((st = check_source(c, sources[i], len, &log_k[i])) != JB_OK) return st;
+            for (size_t k = 0; k < i; ++k)
+                if (sources[i].type == JB_SOURCE_TABLE && sources[k].type == JB_SOURCE_TABLE && sources[k].table == sources[i].table)
+                    return c->fail(JB_ERR_INVALID, "member: duplicate table handle");
+        }
+        // everything is allocated here: the columns, the eq tables, the len/2 outputs, the LowToHigh ping-pong buffers
+        mem = new (std::nothrow) jb_member();
+        if (!mem) return JB_ERR_OOM;
+        mem->ctx = c;
+        mem->m = D;
+        mem->order = order;
+        mem->len = len;
+        mem->rounds = 0;
+        while (((size_t)1 << mem->rounds) < len) ++mem->rounds;
+        make_expr(mem, monomials, nmonomials, nsources, D);
+        mem->tables.resize(nsources);
+        mem->src.resize(nsources);
+        unsigned int* d_flag = nullptr;
+        st = c->dev_alloc((void**)&d_flag, sizeof(unsigned int));
+        if (st == JB_OK) st = c->check(cudaMemsetAsync(d_flag, 0, sizeof(unsigned int), c->stream), "expr sources: flag memset");
+        for (size_t i = 0; i < nsources && st == JB_OK; ++i) {
+            const jb_source& sr = sources[i];
+            SourceCol& sc = mem->src[i];
+            sc.type = sr.type;
+            if (sr.type == JB_SOURCE_TABLE) continue;
+            sc.kind = sr.kind;
+            sc.K = (uint32_t)sr.K;
+            Table& t = mem->tables[i];
+            st = c->dev_alloc((void**)&t.buf, len / 2 * 32);
+            if (st != JB_OK) break;
+            t.cap = len / 2;
+            t.len = len;
+            if (order == JB_LOW_TO_HIGH && (st = c->ensure_alt(t, std::max<size_t>(len / 4, 1))) != JB_OK) break;
+            st = sources_copy_column(c, sr.values, len * (size_t)small_kind_bytes(sr.kind), sr.on_device, &sc.values);
+            if (st == JB_OK && sr.type == JB_SOURCE_ONE_HOT) st = sources_one_hot_eq(c, sc, len, sr.r_addr, log_k[i], d_flag);
+        }
+        unsigned int flag = 0;
+        if (st == JB_OK) st = c->check(cudaMemcpyAsync(&flag, d_flag, sizeof flag, cudaMemcpyDeviceToHost, c->stream),
+                                       "expr sources: flag D2H");
+        // (the caller's columns are borrowed for the call only)
+        if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "expr sources: creation sync");
+        if (st == JB_OK && flag) st = c->fail(JB_ERR_INVALID, "one-hot: an address >= K that is not the none value");
+        c->dev_free(d_flag);
+        if (st != JB_OK) {
+            discard_sources(mem);
+            return st;
+        }
+        for (size_t i = 0; i < nsources; ++i) {  // ownership of the table sources moves into the member
+            if (sources[i].type != JB_SOURCE_TABLE) continue;
+            auto it = c->tables.find(sources[i].table);
+            mem->tables[i] = it->second;
+            c->tables.erase(it);
+            if (order == JB_LOW_TO_HIGH && st == JB_OK) st = c->ensure_alt(mem->tables[i], len / 2);
+        }
+    }
+    if (st != JB_OK) {
+        jb_member_destroy(mem);
+        *out = nullptr;
+        return st;
+    }
+    *out = mem;
+    return eq_w_or_null ? eq_setup(mem, eq_w_or_null, nvars, eq_scale_or_null, out) : JB_OK;
 }
 
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
@@ -1195,6 +1341,8 @@ int jb_member_export_table(jb_member* mem, size_t j, void* device_dst, size_t ca
     Guard g(c, true);
     before_launch(mem);  // the host's view of the tables (buffer parity, length) is exact at a round boundary
     if (j >= (size_t)mem->ntables()) return c->fail(JB_ERR_INVALID, "export_table: table index out of range");
+    if (!mem->src.empty() && mem->src[j].type != JB_SOURCE_TABLE)
+        return c->fail(JB_ERR_INVALID, "export_table: the source is not bound yet (a column, not a field table)");
     if (cap_elems < mem->len) return c->fail(JB_ERR_INVALID, "export_table: destination too small");
     if (len_out) *len_out = mem->len;
     return c->check(cudaMemcpyAsync(device_dst, mem->tables[j].buf, mem->len * 32, cudaMemcpyDeviceToDevice, c->stream),
@@ -1223,9 +1371,14 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
         return resident_member_final(mem, bind);
     }
     before_launch(mem);
-    for (int j = 0; j < mem->ntables(); ++j) {
-        int st = bind_table(c, mem->tables[j], bind, mem->order);
+    if (!mem->src.empty()) {  // len = 2: the sources are bound straight from their columns
+        int st = sources_finish(mem, bind);
         if (st != JB_OK) return st;
+    } else {
+        for (int j = 0; j < mem->ntables(); ++j) {
+            int st = bind_table(c, mem->tables[j], bind, mem->order);
+            if (st != JB_OK) return st;
+        }
     }
     mem->len /= 2;
     return JB_OK;
@@ -1269,6 +1422,7 @@ void jb_member_destroy(jb_member* mem) {
     Guard g(mem->ctx, true);
     if (mem->run) resident_end(mem->run, false);
     if (mem->eq_tabs) mem->ctx->dev_free(mem->eq_tabs);
+    sources_release(mem);
     for (auto& t : mem->tables) mem->ctx->release(t);
     delete mem;
 }

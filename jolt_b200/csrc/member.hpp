@@ -50,6 +50,15 @@ struct WaitAcc {
 
 }  // namespace jbi
 
+// A source of an expression member before its bind (jb_member_create_expr_sources): what the source pass reads.
+struct SourceCol {
+    int type = JB_SOURCE_TABLE;
+    int kind = 0;
+    void* values = nullptr;    // member-owned copy of the column (COMPACT / ONE_HOT)
+    uint64_t* eq = nullptr;    // ONE_HOT: eq(r_addr, .), K entries
+    uint32_t K = 0;
+};
+
 // One ProveRounds member on the device (~ Box<dyn SumcheckKernel>): the relation
 //   sum_x sum_{k<P} prod_{j<D} f_{kD+j}(x)       (degree D, T = D * P dense tables)
 // optionally weighted by a split eq polynomial, optionally index-sharded over ranks.
@@ -95,8 +104,25 @@ struct jb_member {
     // largest monomial degree, `terms` unused); it never runs in a resident kernel
     bool expr = false;
     jb::ExprParams ex;
+    // expression member over sources (jb_member_create_expr_sources): until the sources are bound, src[j] describes
+    // table j - a compact or one-hot source reads its member-owned column and its Table's buffer is where the bind
+    // writes the len/2 field entries. Cleared (and the columns released) by the bind.
+    std::vector<SourceCol> src;
     int ntables() const { return expr ? ex.ntables : m * terms; }
 };
+
+// sources.cu -------------------------------------------------------------------------------------------------
+// The source pass of rounds 0 (bind == false) and 1 (bind: the sources are bound into their Tables' buffers, field
+// tables as tp says). ex carries the round's points.
+int sources_round(jb_ctx* c, const jb_member* mem, bool weighted, const jb::TablePtrs& tp, size_t pairs, bool bind,
+                  const jb::BindScalar& s, const jb::ExprParams& ex, jb::RoundOut out);
+// The terminal bind of a member whose sources are still unbound (len = 2): every table and source to one entry.
+int sources_finish(jb_member* mem, const uint64_t r[4]);
+// Releases the columns and eq tables of the sources (after their bind, or when the member is destroyed).
+void sources_release(jb_member* mem);
+// Member-owned device copy of a column (host or device memory), and the one-hot eq table with the address check.
+int sources_copy_column(jb_ctx* c, const void* values, size_t bytes, int on_device, void** out);
+int sources_one_hot_eq(jb_ctx* c, SourceCol& s, size_t len, const uint64_t* r_addr, size_t log_k, unsigned int* d_flag);
 
 // resident.cu ------------------------------------------------------------------------------------------------
 // Starts a resident kernel serving `n` members (same D, P, order, same context; n <= RES_MAX_MEMBERS). Members

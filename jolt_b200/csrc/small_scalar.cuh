@@ -94,4 +94,13 @@ __device__ __forceinline__ bool ld_small(const void* values, size_t i, int kind,
     return neg;
 }
 
+// F::from(v) of a value as ld_small returns it (canonical Montgomery form)
+__device__ __forceinline__ Fr promote_small(const uint32_t mag[4], bool neg) {
+    Fr k = Fr::zero();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) k.v[j] = mag[j];
+    Fr m = fp_to_mont(k);  // |v| < 2^128 < r: already canonical as an integer
+    return neg ? fp_neg(m) : m;
+}
+
 }  // namespace jb
