@@ -447,6 +447,43 @@ int jb_one_hot_evaluate(jb_ctx* ctx, const void* const* columns, size_t count, i
 int jb_one_hot_pushforward(jb_ctx* ctx, const void* const* columns, size_t count, int kind, size_t T, size_t K,
                            int on_device, const uint64_t* r_cycle, jb_table* out_tables);
 
+/* ---- random linear combinations for batched openings ---------------------------------------------------------------
+ * A NEW resident table of len entries (len a power of two):
+ *   P[x] = sum_i c_i p_i[x]   for x < len_i,   and p_i contributes 0 for x >= len_i.
+ * A term shorter than len is the PREFIX of the index range (its high variables are zero): with point[0] <-> the MSB,
+ * P(point) = sum_i c_i prod_{k < n - n_i} (1 - point[k]) p_i(point[n - n_i ..]), and for HyperKZG
+ * commit(P) = sum_i c_i commit(p_i) exactly, since the bases are prefixes too. The terms:
+ *  - JB_LC_TABLE: a resident field table, borrowed and not modified (the same handle may appear more than once);
+ *    len_i = the table's length.
+ *  - JB_LC_COMPACT: len_i = `len` integers of `kind` (any jb_scalar_kind but JB_SCALAR_FR), value F::from(v) as in
+ *    jb_table_upload_small.
+ *  - JB_LC_ONE_HOT: the 0/1 polynomial jb_msm_g1_one_hot_rows commits and jb_one_hot_evaluate evaluates, from an
+ *    address column of T = `len` entries of `kind` (JB_SCALAR_U8 / U16, the all-ones value is the none value) and
+ *    `layout`; len_i = K T.
+ * coeff: canonical Montgomery limbs (125-bit [0,0,lo,hi] challenges and full values alike). Columns are host memory
+ * borrowed for the call (on_device = 0) or caller-owned device memory read in place (1, e.g. torch tensors). One pass
+ * writes each output entry once and reads each term once in its own format; the output is canonical, bit-exact and
+ * deterministic. Errors, before anything is allocated: JB_ERR_INVALID for a null pointer, count == 0, an unknown type,
+ * kind or layout, len, a term length, K or T that is not a power of two, a term longer than len, an unknown table
+ * handle, a non-canonical coefficient, on_device not 0 / 1, a misaligned device column; JB_ERR_UNSUPPORTED beyond
+ * one-hot T < 2^31, K <= 2^16, count < 2^32. A one-hot address >= K that is not the none value is found on the device
+ * and returns JB_ERR_INVALID: no table is created, nothing stays allocated and the context stays usable. */
+#define JB_LC_TABLE 0
+#define JB_LC_COMPACT 1
+#define JB_LC_ONE_HOT 2
+typedef struct jb_lc_term {
+    int type;              /* JB_LC_* */
+    int kind;              /* COMPACT: any kind but JB_SCALAR_FR; ONE_HOT: JB_SCALAR_U8 / U16 */
+    int on_device;         /* COMPACT / ONE_HOT: 0 host memory, 1 caller-owned device memory */
+    int layout;            /* ONE_HOT: JB_ONE_HOT_CYCLE_MAJOR / JB_ONE_HOT_ADDRESS_MAJOR */
+    jb_table table;        /* TABLE */
+    const void* values;    /* COMPACT: len entries; ONE_HOT: T addresses */
+    size_t len;            /* COMPACT: entries; ONE_HOT: T (cycles); TABLE: ignored (the table's length) */
+    size_t K;              /* ONE_HOT */
+    uint64_t coeff[4];     /* canonical Montgomery limbs */
+} jb_lc_term;
+int jb_table_linear_combination(jb_ctx* ctx, const jb_lc_term* terms, size_t count, size_t len, jb_table* out);
+
 /* Batch affine addition: batch_g1_additions_multi_affine (crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150),
  * the one-hot / binary column path of Dory's tier-1 commitments (crates/jolt-dory/src/streaming.rs:68,128,152,201).
  * Set s is indices[set_offsets[s] .. set_offsets[s + 1]) into `bases`; out_xy receives one AFFINE point per set

@@ -23,6 +23,7 @@ from .api import (  # noqa: F401
     G1Bases,
     HyperKZG,
     HyperKZGProof,
+    LinearTerm,
     Polynomial,
     ProductMember,
     ProvedBatch,

@@ -100,6 +100,7 @@ SIGNATURES = {
                                            ctypes.c_int, ctypes.c_int, c_u64p, c_u64p]),
     "jb_one_hot_pushforward": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, c_size_t,
                                               c_size_t, ctypes.c_int, c_u64p, c_u64p]),
+    "jb_table_linear_combination": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_u64p]),
     "jb_ctx_diag": (ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_double)]),
     "jb_ctx_run_log": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.POINTER(c_size_t)]),
     "jb_ctx_timing_enable": (ctypes.c_int, [c_void_p, ctypes.c_int, ctypes.c_uint64]),
@@ -149,6 +150,15 @@ JB_SOURCE_TABLE, JB_SOURCE_COMPACT, JB_SOURCE_ONE_HOT = 0, 1, 2
 class SourceC(ctypes.Structure):
     _fields_ = [("type", ctypes.c_int), ("kind", ctypes.c_int), ("on_device", ctypes.c_int), ("table", ctypes.c_uint64),
                 ("values", c_void_p), ("K", c_size_t), ("r_addr", c_u64p)]
+
+
+JB_LC_TABLE, JB_LC_COMPACT, JB_LC_ONE_HOT = 0, 1, 2
+
+
+class LcTermC(ctypes.Structure):
+    _fields_ = [("type", ctypes.c_int), ("kind", ctypes.c_int), ("on_device", ctypes.c_int), ("layout", ctypes.c_int),
+                ("table", ctypes.c_uint64), ("values", c_void_p), ("len", c_size_t), ("K", c_size_t),
+                ("coeff", ctypes.c_uint64 * 4)]
 
 
 class FinishWorkC(ctypes.Structure):

@@ -247,6 +247,23 @@ class Polynomial:
         return Polynomial.batch_evaluate([self], point)[0]
 
     @staticmethod
+    def linear_combination(session: Session, terms: list["LinearTerm"], length: int | None = None) -> "Polynomial":
+        """P = sum_i c_i p_i as a new device polynomial of `length` entries (a power of two; default: the longest
+        term) in one pass over the terms in their own formats (jb_table_linear_combination) - the joint polynomial of
+        a batched opening. A shorter term is the prefix of the index range (its high variables are zero)."""
+        if not terms:
+            raise ValueError("linear_combination: at least one term")
+        n = max(t.length for t in terms) if length is None else length
+        arr = (_lib.LcTermC * len(terms))()
+        keep = []
+        for i, t in enumerate(terms):
+            t._fill(arr[i], keep)
+        h = ctypes.c_uint64()
+        session.check(session.lib.jb_table_linear_combination(session.h, ctypes.cast(arr, ctypes.c_void_p), len(terms),
+                                                              n, ctypes.byref(h)))
+        return Polynomial(session, h.value)
+
+    @staticmethod
     def batch_evaluate(polys: list["Polynomial"], point) -> list[int]:
         """Every polynomial (one session, one length 2^len(point)) at the same point, in one pass per table."""
         if not polys:
@@ -793,6 +810,52 @@ class Source:
         c.K = self.K
         if self.r_addr is not None and self.r_addr.shape[0]:
             c.r_addr = _p(self.r_addr)
+        keep.append(self)
+
+
+class LinearTerm:
+    """One term c p of Polynomial.linear_combination. Build with LinearTerm.table / compact / one_hot; `coeff` is a
+    Python int (taken mod r) or 4 Montgomery limbs. Columns are borrowed for the call (host arrays are copied to the
+    device for it, CUDA tensors are read in place)."""
+
+    def __init__(self, type_: int, length: int, coeff, poly: Polynomial | None = None, ptr: int = 0, kind: int = 0,
+                 on_device: int = 0, layout: int = 0, T: int = 0, K: int = 0, keep=None):
+        self.type, self.length, self.poly, self.ptr, self.kind = type_, length, poly, ptr, kind
+        self.on_device, self.layout, self.T, self.K, self.keep = on_device, layout, T, K, keep
+        self.coeff = _limbs(coeff % F.R_MOD if isinstance(coeff, (int, np.integer)) else coeff)
+
+    @classmethod
+    def table(cls, poly: Polynomial, coeff) -> "LinearTerm":
+        """A device field polynomial; it is read, not modified or taken over."""
+        return cls(_lib.JB_LC_TABLE, len(poly), coeff, poly=poly)
+
+    @classmethod
+    def compact(cls, values, coeff, kind: str | None = None) -> "LinearTerm":
+        """A compact integer column (Polynomial<T>) with value F::from(v), taken as Source.compact takes it."""
+        s = Source.compact(values, kind)
+        return cls(_lib.JB_LC_COMPACT, s.length, coeff, ptr=s.ptr, kind=s.kind, on_device=s.on_device, T=s.length,
+                   keep=s.keep)
+
+    @classmethod
+    def one_hot(cls, addresses, K: int, coeff, layout: str = "cycle_major") -> "LinearTerm":
+        """The one-hot polynomial of G1Bases.one_hot_rows / one_hot_evaluate (K T entries, coefficient (k, j) = 1 iff
+        addresses[j] == k at flat index j K + k "cycle_major" or k T + j "address_major") from its address column: a
+        uint8 / uint16 numpy array or CUDA tensor whose all-ones value is the none value."""
+        if layout not in ONE_HOT_LAYOUTS:
+            raise ValueError(f"LinearTerm.one_hot: layout must be one of {sorted(ONE_HOT_LAYOUTS)}")
+        ptrs, kind, T, dev, keep = _address_columns(addresses, "LinearTerm.one_hot")
+        if len(ptrs) != 1:
+            raise ValueError("LinearTerm.one_hot: one address column")
+        return cls(_lib.JB_LC_ONE_HOT, K * T, coeff, ptr=ptrs[0], kind=kind, on_device=dev,
+                   layout=ONE_HOT_LAYOUTS[layout], T=T, K=K, keep=keep)
+
+    def _fill(self, c, keep: list):
+        c.type, c.kind, c.on_device, c.layout = self.type, self.kind, self.on_device, self.layout
+        if self.poly is not None:
+            c.table = self.poly.handle
+        c.values = self.ptr or None
+        c.len, c.K = self.T, self.K
+        c.coeff[:] = [int(x) for x in self.coeff]
         keep.append(self)
 
 

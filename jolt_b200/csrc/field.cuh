@@ -487,6 +487,36 @@ __device__ __forceinline__ void mul_wide_acc_reg(uint32_t (&A)[17], const uint32
           "r"(O[9]), "r"(O[10]), "r"(O[11]), "r"(O[12]), "r"(O[13]), "r"(O[14]));
 }
 
+// A[0..16] += a * b for a multiplier of BW 32-bit words (BW = 8: the full product of mul_wide_acc_reg). The partial
+// products are laid out as in mul_wide_acc_reg (E: pairs at even limb positions, O: shifted by one limb).
+template <int BW>
+__device__ __forceinline__ void mul_wide_acc_bw(uint32_t (&A)[17], const uint32_t* a, const uint32_t* b) {
+    if (BW == 8) {
+        mul_wide_acc_reg(A, a, b);
+        return;
+    }
+    uint32_t E[17], O[17];
+#pragma unroll
+    for (int k = 0; k < 17; ++k) E[k] = O[k] = 0;
+#pragma unroll
+    for (int i = 0; i < BW; ++i) {
+        if ((i & 1) == 0) {
+            chain8_top(E + i, E[i + 8], a[0], a[2], a[4], a[6], b[i]);
+            chain8_top(O + i, O[i + 8], a[1], a[3], a[5], a[7], b[i]);
+        } else {
+            chain8_top(O + i - 1, O[i + 7], a[0], a[2], a[4], a[6], b[i]);
+            chain8_top(E + i + 1, E[i + 9], a[1], a[3], a[5], a[7], b[i]);
+        }
+    }
+    uint64_t carry = 0;
+#pragma unroll
+    for (int k = 0; k < 17; ++k) {
+        const uint64_t t = (uint64_t)A[k] + E[k] + (k ? O[k - 1] : 0u) + carry;
+        A[k] = (uint32_t)t;
+        carry = t >> 32;
+    }
+}
+
 // 544-bit accumulator (17 words at acc[k * stride]) -> canonical acc * R^-1 mod p. It sits on the latency path of
 // every sumcheck round (one lane per value reduces the block's column sums), so it is three Montgomery products on
 // the fast IMAD.WIDE rows instead of a word-serial 64-bit loop: with acc = lo + hi R + top R^2 (R = 2^256),

@@ -37,6 +37,29 @@ inline bool canonical_fr(const uint64_t r[4]) { return !HostFr::geq_p(r); }
 int bind_table(jb_ctx* c, Table& t, const uint64_t r[4], int order);  // Polynomial::bind_with_order on one table
 int eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, uint64_t* d_out);
 
+// Columns of a call that reads them in place (mle_eval.cu, lincomb.cu): host columns are copied to device memory
+// allocated for the call and freed with it; device columns are used as they are.
+struct Columns {
+    jb_ctx* c;
+    std::vector<void*> owned;
+    explicit Columns(jb_ctx* ctx) : c(ctx) {}
+    ~Columns() {
+        for (void* p : owned) c->dev_free(p);
+    }
+    int get(const void* src, size_t bytes, int on_device, const void** dst) {
+        if (on_device) {
+            *dst = src;
+            return JB_OK;
+        }
+        void* d = nullptr;
+        int st = c->dev_alloc(&d, bytes);
+        if (st != JB_OK) return st;
+        owned.push_back(d);
+        *dst = d;
+        return c->check(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream), "column H2D");
+    }
+};
+
 // Accumulates the host time spent waiting for a round result (jb_ctx_diag).
 struct WaitAcc {
     jb_ctx* c;

@@ -47,36 +47,6 @@ struct EvalCol {  // one output of a launch: its source and its lane block
     uint64_t out;
 };
 
-// A[0..16] += a * b for a multiplier of BW 32-bit words (BW = 8: the full product of mul_wide_acc_reg). The partial
-// products are laid out as in mul_wide_acc_reg (E: pairs at even limb positions, O: shifted by one limb).
-template <int BW>
-__device__ __forceinline__ void mul_wide_acc_bw(uint32_t (&A)[17], const uint32_t* a, const uint32_t* b) {
-    if (BW == 8) {
-        mul_wide_acc_reg(A, a, b);
-        return;
-    }
-    uint32_t E[17], O[17];
-#pragma unroll
-    for (int k = 0; k < 17; ++k) E[k] = O[k] = 0;
-#pragma unroll
-    for (int i = 0; i < BW; ++i) {
-        if ((i & 1) == 0) {
-            chain8_top(E + i, E[i + 8], a[0], a[2], a[4], a[6], b[i]);
-            chain8_top(O + i, O[i + 8], a[1], a[3], a[5], a[7], b[i]);
-        } else {
-            chain8_top(O + i - 1, O[i + 7], a[0], a[2], a[4], a[6], b[i]);
-            chain8_top(E + i + 1, E[i + 9], a[1], a[3], a[5], a[7], b[i]);
-        }
-    }
-    uint64_t carry = 0;
-#pragma unroll
-    for (int k = 0; k < 17; ++k) {
-        const uint64_t t = (uint64_t)A[k] + E[k] + (k ? O[k - 1] : 0u) + carry;
-        A[k] = (uint32_t)t;
-        carry = t >> 32;
-    }
-}
-
 // ---- value loaders: A += e * v(i) -----------------------------------------------------------------------------------
 struct FieldSrc {
     static constexpr int SMEM_U4 = 1;
@@ -371,28 +341,6 @@ int launch_small(EvalPlan& p, int kind, size_t first, size_t n) {
         default: return launch_eval(p, SmallSrc<SK_S128>{}, first, n);
     }
 }
-
-// Host columns are copied to the device for the call; device columns are used in place.
-struct Columns {
-    jb_ctx* c;
-    std::vector<void*> owned;
-    explicit Columns(jb_ctx* ctx) : c(ctx) {}
-    ~Columns() {
-        for (void* p : owned) c->dev_free(p);
-    }
-    int get(const void* src, size_t bytes, int on_device, const void** dst) {
-        if (on_device) {
-            *dst = src;
-            return JB_OK;
-        }
-        void* d = nullptr;
-        int st = c->dev_alloc(&d, bytes);
-        if (st != JB_OK) return st;
-        owned.push_back(d);
-        *dst = d;
-        return c->check(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream), "evaluate column H2D");
-    }
-};
 
 int check_one_hot(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K, int on_device,
                   const char* what) {
