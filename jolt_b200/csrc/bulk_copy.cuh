@@ -1,5 +1,5 @@
 // Bulk asynchronous copies global -> shared (cp.async.bulk, SASS UBLKCP) tracked by shared-memory mbarriers: the
-// primitives of the TMA-staged sweeps (tma_ab.cuh, the resident kernel's staged pass in resident.cuh).
+// primitives of the resident kernel's staged pass (resident.cuh).
 #pragma once
 #include <cstdint>
 

@@ -18,7 +18,6 @@
 #include "resident.cuh"
 #include "small_scalar.cuh"
 #include "sumcheck_host.hpp"
-#include "tma_ab.cuh"
 
 using namespace jb;
 using namespace jbi;
@@ -30,127 +29,41 @@ constexpr int JB_SLOT_U64 = 128;
 
 namespace {
 
-template <int M, int P, int ORDER, bool BIND, bool HI4, bool SKIP1, int BLOCK, int MINB>
-int launch_fused_mb(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, RoundOut out) {
-    auto kernel = fused_round_kernel<M, P, ORDER, BIND, HI4, SKIP1, BLOCK, MINB>;
-    constexpr size_t smem = FusedShape<M, SKIP1>::smem_bytes(BLOCK);
-    static int per_sm = [&] {
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int nb = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, BLOCK, smem) != cudaSuccess || nb < 1) nb = 1;
-        return nb;
-    }();
-    // grid-stride over whole waves of resident blocks; tiny rounds take one (small) block
-    size_t need = (pairs + BLOCK - 1) / BLOCK;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    if (grid < 1) grid = 1;
-    constexpr int K = FusedShape<M, SKIP1>::K;
-    int st = c->ensure_partial(grid * K);
-    if (st != JB_OK) return st;
-    out.partial = c->d_partial;
-    int tix = c->timing_begin(BIND ? 0 : 2, pairs, M * P);
-    // latency path: a round of <= 32 pairs runs as one warp (no barriers, no shared-memory stage)
-    const unsigned block = pairs <= 32 ? 32u : (unsigned)BLOCK;
-    kernel<<<(unsigned)grid, block, smem, c->stream>>>(tp, pairs, s, out);
-    c->timing_end(tix);
-    c->launches++;
-    return c->check(cudaGetLastError(), "fused_round_kernel launch");
-}
-
-// A/B (JB_EVAL_TMA=1): the degree-2 eval-only sweep with its evaluation blocks staged by the TMA unit (tma_ab.cuh)
-template <int ORDER>
-int launch_eval2_tma(jb_ctx* c, const TablePtrs& tp, size_t pairs, RoundOut out) {
-    auto kernel = eval2_tma_kernel<ORDER>;
-    constexpr size_t smem = TmaShape::smem_bytes;
-    static int per_sm = [&] {
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int nb = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, TMA_THREADS, smem) != cudaSuccess || nb < 1) nb = 1;
-        return nb;
-    }();
-    size_t need = (pairs + TMA_TILE - 1) / TMA_TILE;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    if (grid < 1) grid = 1;
-    int st = c->ensure_partial(grid * 2);
-    if (st != JB_OK) return st;
-    out.partial = c->d_partial;
-    int tix = c->timing_begin(2, pairs, 2);
-    kernel<<<(unsigned)grid, TMA_THREADS, smem, c->stream>>>(tp, pairs, out);
-    c->timing_end(tix);
-    c->launches++;
-    return c->check(cudaGetLastError(), "eval2_tma_kernel launch");
-}
-
-template <int M, int P, int ORDER, bool BIND, bool HI4, bool SKIP1>
+// WEIGHTED: a split-eq member's pass (SKIP1: s(1) comes from the claim)
+template <int M, int P, int ORDER, bool BIND, bool HI4, bool SKIP1, bool WEIGHTED>
 int launch_fused(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, const RoundOut& out) {
-    if constexpr (M == 2 && P == 1 && !BIND && SKIP1) {
-        if (c->eval_tma && pairs >= 4096) return launch_eval2_tma<ORDER>(c, tp, pairs, out);
-    }
-    // occupancy shapes (tuning knob JB_FUSED_SHAPE): 0 = 256 threads x 2 blocks (128 registers),
-    // 1 = 128 threads x 5 blocks (<= 102 registers, 20 warps/SM)
-    if constexpr (M == 2 && P == 1) {
-        if (c->fused_shape == 1) return launch_fused_mb<M, P, ORDER, BIND, HI4, SKIP1, 128, 5>(c, tp, pairs, s, out);
-    }
-    return launch_fused_mb<M, P, ORDER, BIND, HI4, SKIP1, 256, 2>(c, tp, pairs, s, out);
-}
-
-// weighted (split-eq) passes: s(1) from the claim, 256 x 2
-template <int M, int ORDER, bool BIND, bool HI4>
-int launch_weighted(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, RoundOut out) {
-    auto kernel = fused_round_kernel<M, 1, ORDER, BIND, HI4, true, 256, 2, true>;
-    constexpr size_t smem = FusedShape<M, true>::smem_bytes(256);
+    auto kernel = fused_round_kernel<M, P, ORDER, BIND, HI4, SKIP1, WEIGHTED>;
+    constexpr size_t smem = FusedShape<M, SKIP1>::smem_bytes(FUSED_BLOCK);
     static int per_sm = [&] {
         cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         int nb = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, 256, smem) != cudaSuccess || nb < 1) nb = 1;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, FUSED_BLOCK, smem) != cudaSuccess || nb < 1) nb = 1;
         return nb;
     }();
-    size_t need = (pairs + 255) / 256;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    if (grid < 1) grid = 1;
-    int st = c->ensure_partial(grid * M);
-    if (st != JB_OK) return st;
-    out.partial = c->d_partial;
-    int tix = c->timing_begin(BIND ? 0 : 2, pairs, M);
-    const unsigned block = pairs <= 32 ? 32u : 256u;
-    kernel<<<(unsigned)grid, block, smem, c->stream>>>(tp, pairs, s, out);
-    c->timing_end(tix);
-    c->launches++;
-    return c->check(cudaGetLastError(), "fused_round_kernel (weighted) launch");
+    return launch_round(c, kernel, FUSED_BLOCK, smem, per_sm, pairs, FusedShape<M, SKIP1>::K, BIND ? 0 : 2, M * P,
+                        WEIGHTED ? "fused_round_kernel (weighted) launch" : "fused_round_kernel launch", out, tp, pairs, s);
 }
 
-template <int M, int ORDER>
-int dispatch_weighted1(jb_ctx* c, const TablePtrs& tp, size_t pairs, bool bind, bool hi4, const BindScalar& s,
-                       const RoundOut& out) {
-    if (!bind) return launch_weighted<M, ORDER, false, false>(c, tp, pairs, s, out);
-    return hi4 ? launch_weighted<M, ORDER, true, true>(c, tp, pairs, s, out)
-               : launch_weighted<M, ORDER, true, false>(c, tp, pairs, s, out);
+template <int M, int P, int ORDER, bool SKIP1, bool WEIGHTED = false>
+int dispatch_fused2(jb_ctx* c, const TablePtrs& tp, size_t pairs, bool bind, bool hi4, const BindScalar& s,
+                    const RoundOut& out) {
+    if (!bind) return launch_fused<M, P, ORDER, false, false, SKIP1, WEIGHTED>(c, tp, pairs, s, out);
+    return hi4 ? launch_fused<M, P, ORDER, true, true, SKIP1, WEIGHTED>(c, tp, pairs, s, out)
+               : launch_fused<M, P, ORDER, true, false, SKIP1, WEIGHTED>(c, tp, pairs, s, out);
 }
 
 int dispatch_weighted(jb_ctx* c, int m, int order, const TablePtrs& tp, size_t pairs, bool bind, bool hi4, const BindScalar& s,
                       const RoundOut& out) {
     const bool l2h = order == JB_LOW_TO_HIGH;
     switch (m) {
-        case 1: return l2h ? dispatch_weighted1<1, ORDER_LOW_TO_HIGH>(c, tp, pairs, bind, hi4, s, out)
-                           : dispatch_weighted1<1, ORDER_HIGH_TO_LOW>(c, tp, pairs, bind, hi4, s, out);
-        case 2: return l2h ? dispatch_weighted1<2, ORDER_LOW_TO_HIGH>(c, tp, pairs, bind, hi4, s, out)
-                           : dispatch_weighted1<2, ORDER_HIGH_TO_LOW>(c, tp, pairs, bind, hi4, s, out);
-        case 3: return l2h ? dispatch_weighted1<3, ORDER_LOW_TO_HIGH>(c, tp, pairs, bind, hi4, s, out)
-                           : dispatch_weighted1<3, ORDER_HIGH_TO_LOW>(c, tp, pairs, bind, hi4, s, out);
+        case 1: return l2h ? dispatch_fused2<1, 1, ORDER_LOW_TO_HIGH, true, true>(c, tp, pairs, bind, hi4, s, out)
+                           : dispatch_fused2<1, 1, ORDER_HIGH_TO_LOW, true, true>(c, tp, pairs, bind, hi4, s, out);
+        case 2: return l2h ? dispatch_fused2<2, 1, ORDER_LOW_TO_HIGH, true, true>(c, tp, pairs, bind, hi4, s, out)
+                           : dispatch_fused2<2, 1, ORDER_HIGH_TO_LOW, true, true>(c, tp, pairs, bind, hi4, s, out);
+        case 3: return l2h ? dispatch_fused2<3, 1, ORDER_LOW_TO_HIGH, true, true>(c, tp, pairs, bind, hi4, s, out)
+                           : dispatch_fused2<3, 1, ORDER_HIGH_TO_LOW, true, true>(c, tp, pairs, bind, hi4, s, out);
         default: return c->fail(JB_ERR_UNSUPPORTED, "eq member: m must be 1..3");
     }
-}
-
-
-template <int M, int P, int ORDER, bool SKIP1>
-int dispatch_fused2(jb_ctx* c, const TablePtrs& tp, size_t pairs, bool bind, bool hi4, const BindScalar& s,
-                    const RoundOut& out) {
-    if (!bind) return launch_fused<M, P, ORDER, false, false, SKIP1>(c, tp, pairs, s, out);
-    return hi4 ? launch_fused<M, P, ORDER, true, true, SKIP1>(c, tp, pairs, s, out)
-               : launch_fused<M, P, ORDER, true, false, SKIP1>(c, tp, pairs, s, out);
 }
 
 template <int M, int P>
@@ -181,7 +94,7 @@ int dispatch_fused(jb_ctx* c, int m, int terms, int order, bool skip1, const Tab
 
 // expression members (expr_pass.cuh): EXPR_BLOCK threads per block, shared memory by the member's table count
 template <int ORDER, bool BIND, bool HI4, bool WEIGHTED>
-int launch_expr(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, const ExprParams& ex, RoundOut out) {
+int launch_expr(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, const ExprParams& ex, const RoundOut& out) {
     auto kernel = expr_round_kernel<ORDER, BIND, HI4, WEIGHTED>;
     static const bool attr = [&] {
         cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)expr_smem_bytes(EXPR_MAX_TABLES));
@@ -196,19 +109,8 @@ int launch_expr(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& 
             per_sm = 1;
         per_sm_by_tables[ex.ntables].store(per_sm, std::memory_order_relaxed);
     }
-    size_t need = (pairs + EXPR_BLOCK - 1) / EXPR_BLOCK;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    if (grid < 1) grid = 1;
-    int st = c->ensure_partial(grid * EXPR_MAX_POINTS);
-    if (st != JB_OK) return st;
-    out.partial = c->d_partial;
-    int tix = c->timing_begin(BIND ? 0 : 2, pairs, ex.D);
-    const unsigned block = pairs <= 32 ? 32u : (unsigned)EXPR_BLOCK;
-    kernel<<<(unsigned)grid, block, smem, c->stream>>>(tp, pairs, s, ex, out);
-    c->timing_end(tix);
-    c->launches++;
-    return c->check(cudaGetLastError(), "expr_round_kernel launch");
+    return launch_round(c, kernel, EXPR_BLOCK, smem, per_sm, pairs, EXPR_MAX_POINTS, BIND ? 0 : 2, ex.D,
+                        "expr_round_kernel launch", out, tp, pairs, s, ex);
 }
 
 template <int ORDER, bool WEIGHTED>
@@ -367,7 +269,7 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
         }
     }
     RoundOut ro;
-    ro.partial = nullptr;  // set by launch_fused
+    ro.partial = nullptr;  // set by launch_round
     ro.counter = c->d_counter;
     ro.lanes = lanes_out ? 1 : 0;
     ro.world = 1;
@@ -1183,8 +1085,7 @@ static int sharded_prove_round(jb_member* mem, const uint64_t* bind, size_t roun
             // the peers' shards and sweeps the gathered tables - no kernel exit, no NCCL call; from here on this
             // member proves its remaining rounds un-sharded (identically on every rank)
             const bool skip1g = claim != nullptr && !c->verify_rounds;
-            if (bind && skip1g && mem->run && len_after == mem->gather_len && resident_gather_fits(c, mem, len_after) &&
-                !std::getenv("JB_NCCL_GATHER")) {
+            if (bind && skip1g && mem->run && len_after == mem->gather_len && resident_gather_fits(c, mem, len_after)) {
                 int st = resident_member_prove(mem, bind, claim, round, false, out_evals, true);
                 if (st == JB_OK) {
                     mem->rounds_done--;  // (the caller counts sharded rounds)

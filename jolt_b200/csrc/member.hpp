@@ -33,6 +33,33 @@ inline BindScalar make_scalar(const uint64_t r[4], bool* hi4) {
 
 inline bool canonical_fr(const uint64_t r[4]) { return !HostFr::geq_p(r); }
 
+// Blocks of `block` threads for a grid-stride pass over `items`: one per `block` items, at most one wave of
+// `per_sm` resident blocks on every SM, at least one.
+inline unsigned launch_grid(const jb_ctx* c, size_t items, int block, int per_sm) {
+    size_t need = (items + block - 1) / block;
+    size_t resident = (size_t)c->sm_count * per_sm;
+    size_t grid = need < resident ? need : resident;
+    return grid < 1 ? 1u : (unsigned)grid;
+}
+
+// Launches one round of a per-round sumcheck kernel over `pairs` pair indices: `kernel(args..., out)`, whose blocks
+// each leave `values` partial sums in the context's partial buffer for the last block to fold. `kind` and `m` label
+// the timed launch (jb_ctx::timing_begin), `what` names a launch error.
+template <typename Kernel, typename... Args>
+int launch_round(jb_ctx* c, Kernel kernel, int block, size_t smem, int per_sm, size_t pairs, int values, int kind, int m,
+                 const char* what, jb::RoundOut out, const Args&... args) {
+    const unsigned grid = launch_grid(c, pairs, block, per_sm);
+    int st = c->ensure_partial((size_t)grid * values);
+    if (st != JB_OK) return st;
+    out.partial = c->d_partial;
+    int tix = c->timing_begin(kind, pairs, m);
+    // latency path: a round of <= 32 pairs runs as one warp (no barriers, no shared-memory stage)
+    kernel<<<grid, pairs <= 32 ? 32u : (unsigned)block, smem, c->stream>>>(args..., out);
+    c->timing_end(tix);
+    c->launches++;
+    return c->check(cudaGetLastError(), what);
+}
+
 // capi.cu
 int bind_table(jb_ctx* c, Table& t, const uint64_t r[4], int order);  // Polynomial::bind_with_order on one table
 int eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, uint64_t* d_out);

@@ -35,14 +35,8 @@ namespace {
 
 // buckets per reduction segment: one thread walks a segment (2 general additions per bucket) and then multiplies the
 // segment's plain sum by its first bucket number (double-and-add, ~330 products): the multiplication is per SEGMENT, so
-// short segments cost work. JB_MSM_SEG overrides (A/B).
+// short segments cost work.
 int msm_seg_size(int buckets) {
-    static const int env = [] {
-        const char* e = getenv("JB_MSM_SEG");
-        const int x = e ? atoi(e) : 0;
-        return x >= 2 && x <= 256 ? x : 0;
-    }();
-    if (env) return env;
     return buckets >= (1 << 21) ? 64 : 16;  // per-segment work shrinks with fewer, longer segments once buckets are many
 }
 
@@ -940,11 +934,7 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
     // wide window's bucket reduction (2^(c-1) buckets) to be in the noise
     // Small MSMs (the tail of HyperKZG's intermediate commitments, verifier-sized MSMs) use a second, tiny
     // table with 8-bit windows over the first bases: 128 buckets, no doubling chain - latency, not work.
-    static const size_t small_max = [] {  // JB_MSM_SMALL_MAX: largest MSM served by the 8-bit-window table (A/B)
-        const char* e = getenv("JB_MSM_SMALL_MAX");
-        const long v = e ? atol(e) : 4096;
-        return (size_t)(v > 0 ? v : 4096);
-    }();
+    constexpr size_t small_max = 4096;  // largest MSM served by the 8-bit-window table
     const bool use_small = by_rows || (srs.pre_small != nullptr && n <= small_max && offset + n <= srs.pre_small_len);
     const bool use_big = !use_small && srs.pre != nullptr && n >= ((size_t)1 << (srs.pre_c - 4));
     const bool shared = use_small || use_big;
@@ -1029,10 +1019,7 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
                     regions = p.W;
                 } else if (p.c - 1 >= 6) {
                     mode = 2;
-                    int rl = 2;  // log2(regions): more rows cost more digit re-reads than their L2 hits save
-                    if (const char* e = getenv("JB_MSM_SCATTER_REGIONS_LOG")) rl = atoi(e);
-                    if (rl < 0) rl = 0;
-                    if (rl > 6) rl = 6;
+                    constexpr int rl = 2;  // log2(regions): more rows cost more digit re-reads than their L2 hits save
                     regions = 1 << rl;
                     range_shift = (unsigned)(p.c - 1) - (unsigned)rl;  // nb = 2^(c-1) buckets
                 }

@@ -540,19 +540,21 @@ __device__ __forceinline__ void fused_pass(const TablePtrs& tp, size_t pairs, co
     __syncthreads();  // scratch is reused by the caller (the last block's fold)
 }
 
-// One launch per round: BLOCK threads per block (256 or 128), MINB = resident blocks per SM requested from
-// ptxas. WEIGHTED: the sweep is sum_y E(y) prod_j(...) with the split-eq weight E(y) = e_out * e_in folded into
+constexpr int FUSED_BLOCK = 256;
+
+// One launch per round: FUSED_BLOCK threads per block, 2 resident blocks per SM (at most 128 registers).
+// WEIGHTED: the sweep is sum_y E(y) prod_j(...) with the split-eq weight E(y) = e_out * e_in folded into
 // table 0's pair AFTER the bound values are stored (GruenSplitEqPolynomial, split_eq.rs:159-447: the eq
 // polynomial is never materialised or bound as a table; its current variable is a linear factor the host
 // multiplies in). Each block writes its sums and the last block folds them (round_epilogue).
-template <int D, int P, int ORDER, bool BIND, bool HI4, bool SKIP1, int BLOCK, int MINB, bool WEIGHTED = false>
-__global__ void __launch_bounds__(BLOCK, MINB) fused_round_kernel(TablePtrs tp, size_t pairs, BindScalar s, RoundOut out) {
+template <int D, int P, int ORDER, bool BIND, bool HI4, bool SKIP1, bool WEIGHTED>
+__global__ void __launch_bounds__(FUSED_BLOCK, 2) fused_round_kernel(TablePtrs tp, size_t pairs, BindScalar s, RoundOut out) {
     constexpr int K = FusedShape<D, SKIP1>::K;
     extern __shared__ uint32_t dsm[];
     Fr acc[K];
-    fused_pass<D, P, ORDER, BIND, HI4, SKIP1, BLOCK, WEIGHTED, true>(
+    fused_pass<D, P, ORDER, BIND, HI4, SKIP1, FUSED_BLOCK, WEIGHTED, true>(
         tp, pairs, s, dsm, (size_t)blockIdx.x * blockDim.x + threadIdx.x, (size_t)gridDim.x * blockDim.x, acc);
-    round_epilogue<K>(acc, dsm + FusedShape<D, SKIP1>::acc_words(BLOCK), out);
+    round_epilogue<K>(acc, dsm + FusedShape<D, SKIP1>::acc_words(FUSED_BLOCK), out);
 }
 
 // ---- eq-table expansion --------------------------------------------------------------------
@@ -650,13 +652,8 @@ static __global__ void __launch_bounds__(256) eq_expand_kernel(const uint64_t* p
 // with a full 254-bit point this kernel is bound by the integer pipe (one Montgomery product per 32 B output),
 // not by HBM.
 // CS: streaming (evict-first) stores - the table is written once and consumed by a LATER kernel; keeping 128 MB+ of
-// it dirty in L2 only evicts what the consumer wants there (A/B: tools/eq_store_probe.py).
-// LOW3: the three register-expanded variables are the LAST three of the point, so a thread's 8 outputs are
-// CONSECUTIVE (256 B; out[(b << 11) | (t << 3) | k] = prefix[b] * mid8[t] * eq3[k], mid8 over the 8 variables before
-// them) instead of 8 KiB apart. Built to test whether the store pattern explains the 2 x DRAM write traffic ncu
-// reports for this kernel: it does not - both layouts, with and without streaming stores, write the same bytes; LOW3
-// is slower and stays off.
-template <bool HI4, bool CS, bool LOW3 = false>
+// it dirty in L2 only evicts what the consumer wants there.
+template <bool HI4, bool CS>
 __global__ void __launch_bounds__(256) eq_stream_kernel(const uint64_t* prefix, const __grid_constant__ EqVars ev,
                                                         const uint64_t* low8, uint64_t* out) {
     const int tid = threadIdx.x;
@@ -672,10 +669,10 @@ __global__ void __launch_bounds__(256) eq_stream_kernel(const uint64_t* prefix, 
             e[2 * i + 1] = hi;
         }
     }
-    const size_t base = ((size_t)blockIdx.x << EQ_BLOCK_VARS) + (LOW3 ? ((size_t)tid << 3) : (size_t)tid);
+    const size_t base = ((size_t)blockIdx.x << EQ_BLOCK_VARS) + (size_t)tid;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-        const size_t idx = base + (LOW3 ? (size_t)k : ((size_t)k << 8));
+        const size_t idx = base + ((size_t)k << 8);
         if (CS) st_elem_cs(out, idx, e[k]);
         else st_elem(out, idx, e[k]);
     }

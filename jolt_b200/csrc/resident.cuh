@@ -46,6 +46,8 @@ constexpr uint64_t RES_THIN_PAIRS = 1ull << 17;  // (2^17: the first thin round 
 // mailbox / accumulator words per member: a thin round returns 8 sums x 17 lanes; a generic round K <= 4 values
 // x 17 lanes (products) or x 8 lanes (D = 1); a terminal bind the T final values x 4 limbs
 constexpr int RES_SLOT_U64 = 136;
+// big passes: this share (%) of the pair range is laid out statically, the rest is claimed by the blocks that are ahead
+constexpr int RES_STATIC_PCT = 75;
 
 // per-member action of a round command (4 bits each, member i at bits [16 + 4i, 20 + 4i) of cmd)
 enum : unsigned { RES_ACT_NONE = 0, RES_ACT_EVAL = 1, RES_ACT_BIND_EVAL = 2, RES_ACT_FINAL = 3 };
@@ -117,7 +119,6 @@ struct ResArgs {
     ResMailbox* mb;     // host-mapped
     ResState* st;       // device
     long long timeout_cycles;
-    int static_pct;     // big passes: this share of the pair range is laid out statically, the rest is claimed (100 = off)
     int staged;         // D = 2, P = 1: large passes run staged_pass (dynamic shared memory >= STG_SMEM_BYTES)
     // peer exchange (world > 1): exchange buffer of every rank as mapped in THIS process
     uint64_t* peer[16];
@@ -754,8 +755,8 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                     const uint32_t ntiles = (uint32_t)(pairs / STG_TILE);
                     // passes of >= 2 tiles per block: the tail of the range is claimed tile by tile
                     uint32_t static_end = ntiles;
-                    if (a.static_pct < 100 && live > 1 && ntiles >= 2 * sh.nblk)
-                        static_end = (uint32_t)((uint64_t)ntiles * (uint64_t)a.static_pct / 100 / sh.nblk * sh.nblk);
+                    if (live > 1 && ntiles >= 2 * sh.nblk)
+                        static_end = (uint32_t)((uint64_t)ntiles * RES_STATIC_PCT / 100 / sh.nblk * sh.nblk);
                     const auto pass = !bind ? staged_pass<ORDER, false, false>
                                       : hi4 ? staged_pass<ORDER, true, true> : staged_pass<ORDER, true, false>;
                     pass(tp, pairs, sc(), reinterpret_cast<uint8_t*>(dsm), b, sh.nblk, static_end, gl, sl);
@@ -766,8 +767,8 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                 const size_t stride = (size_t)sh.nblk * sh.tpb;
                 // passes of >= 2 full sweeps of the grid: the tail of the range is claimed warp by warp
                 tp.static_end = ~(size_t)0;
-                if (a.static_pct < 100 && live > 1 && sh.tpb == RES_BLOCK && (size_t)pairs >= 2 * stride)
-                    tp.static_end = ((size_t)pairs / 100 * (size_t)a.static_pct / stride) * stride;
+                if (live > 1 && sh.tpb == RES_BLOCK && (size_t)pairs >= 2 * stride)
+                    tp.static_end = ((size_t)pairs / 100 * RES_STATIC_PCT / stride) * stride;
                 const auto pass = !bind ? resident_pass<D, P, ORDER, false, false>
                                   : hi4 ? resident_pass<D, P, ORDER, true, true> : resident_pass<D, P, ORDER, true, false>;
                 pass(tp, pairs, sc(), dsm, first, stride, gl, sl);

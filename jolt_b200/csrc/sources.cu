@@ -184,7 +184,7 @@ size_t fill_params(const jb_member* mem, bool staged, SourceParams& sp) {
 
 template <int ORDER, bool BIND, bool HI4, bool WEIGHTED>
 int launch_sources(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScalar& s, const ExprParams& ex,
-                   const SourceParams& sp, size_t smem, RoundOut out) {
+                   const SourceParams& sp, size_t smem, const RoundOut& out) {
     auto kernel = source_round_kernel<ORDER, BIND, HI4, WEIGHTED>;
     static const bool attr = [&] {
         cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SRC_SMEM_MAX);
@@ -195,19 +195,8 @@ int launch_sources(jb_ctx* c, const TablePtrs& tp, size_t pairs, const BindScala
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, EXPR_BLOCK, smem) != cudaSuccess || per_sm < 1)
         per_sm = 1;
-    size_t need = (pairs + EXPR_BLOCK - 1) / EXPR_BLOCK;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    if (grid < 1) grid = 1;
-    int st = c->ensure_partial(grid * EXPR_MAX_POINTS);
-    if (st != JB_OK) return st;
-    out.partial = c->d_partial;
-    int tix = c->timing_begin(BIND ? 0 : 2, pairs, ex.D);
-    const unsigned block = pairs <= 32 ? 32u : (unsigned)EXPR_BLOCK;
-    kernel<<<(unsigned)grid, block, smem, c->stream>>>(tp, pairs, s, ex, sp, out);
-    c->timing_end(tix);
-    c->launches++;
-    return c->check(cudaGetLastError(), "source_round_kernel launch");
+    return launch_round(c, kernel, EXPR_BLOCK, smem, per_sm, pairs, EXPR_MAX_POINTS, BIND ? 0 : 2, ex.D,
+                        "source_round_kernel launch", out, tp, pairs, s, ex, sp);
 }
 
 template <int ORDER, bool WEIGHTED>
