@@ -301,6 +301,24 @@ def _torch_kind(t) -> str | None:
 _KIND_BYTES = {"u8": 1, "u16": 2, "u32": 4, "u64": 8, "u128": 16, "i64": 8, "i128": 16, "s64": 16, "s128": 24}
 
 
+def _compact_column(values, kind: str | None, what: str):
+    """(pointer, jb_scalar_kind, entries, on_device, keep-alive) for one compact column: a numpy array or sequence as
+    small_scalars takes it, or a contiguous CUDA torch tensor (read in place; a 128-bit or sign-magnitude kind is named
+    in `kind` and the tensor holds its raw records)."""
+    if not _is_device_tensor(values):
+        a, k, n = small_scalars(values, kind)
+        return a.ctypes.data, k, n, 0, a
+    if not values.is_contiguous():
+        raise ValueError(f"{what}: device columns must be contiguous")
+    kind = kind or _torch_kind(values)
+    if kind not in _KIND_BYTES:
+        raise ValueError(f"{what}: unsupported device column dtype {values.dtype} (kind={kind})")
+    nbytes = values.numel() * values.element_size()
+    if nbytes % _KIND_BYTES[kind]:
+        raise ValueError(f"{what}: tensor size is not a whole number of entries")
+    return values.data_ptr(), SCALAR_KINDS[kind], nbytes // _KIND_BYTES[kind], 1, values
+
+
 def evaluate_small(session: Session, columns, point, kinds=None) -> list[int]:
     """Compact columns (Polynomial<T>, dense.rs:22-142) evaluated at `point` as the promoted polynomials F::from(v),
     without promoting them (jb_small_evaluate_batch). `columns`: one column or a list of them, all of 2^len(point)
@@ -319,32 +337,13 @@ def evaluate_small(session: Session, columns, point, kinds=None) -> list[int]:
     dev = [_is_device_tensor(c) for c in columns]
     if any(dev) != all(dev):
         raise ValueError("evaluate_small: columns must be all host arrays or all CUDA tensors")
-    keep, ptrs, ks, lens = [], [], [], []
-    for col, kind in zip(columns, kinds):
-        if dev[0]:
-            if not col.is_contiguous():
-                raise ValueError("evaluate_small: device columns must be contiguous")
-            kind = kind or _torch_kind(col)
-            if kind not in _KIND_BYTES:
-                raise ValueError(f"evaluate_small: unsupported device column dtype {col.dtype} (kind={kind})")
-            nbytes = col.numel() * col.element_size()
-            if nbytes % _KIND_BYTES[kind]:
-                raise ValueError("evaluate_small: tensor size is not a whole number of entries")
-            ptrs.append(col.data_ptr())
-            ks.append(SCALAR_KINDS[kind])
-            lens.append(nbytes // _KIND_BYTES[kind])
-        else:
-            a, k, n = small_scalars(col, kind)
-            keep.append(a)
-            ptrs.append(a.ctypes.data)
-            ks.append(k)
-            lens.append(n)
+    ptrs, ks, lens, on_device, _keep = zip(*[_compact_column(c, k, "evaluate_small") for c, k in zip(columns, kinds)])
     if len(set(lens)) != 1:
         raise ValueError("evaluate_small: columns must have one length")
     pt = point_limbs(point)
     out = np.empty((len(columns), 4), dtype=np.uint64)
     session.check(session.lib.jb_small_evaluate_batch(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs),
-                                                      (ctypes.c_int * len(ks))(*ks), lens[0], 1 if dev[0] else 0,
+                                                      (ctypes.c_int * len(ks))(*ks), lens[0], on_device[0],
                                                       _p(pt), pt.shape[0], _p(out)))
     return F.limbs_to_ints(out)
 
@@ -775,19 +774,8 @@ class Source:
         """A compact integer column (Polynomial<T>) with value F::from(v): a numpy array or sequence as small_scalars
         takes it, or a contiguous CUDA tensor (a 128-bit or sign-magnitude kind is named in `kind`, the tensor holding
         its raw records)."""
-        if _is_device_tensor(values):
-            if not values.is_contiguous():
-                raise ValueError("Source.compact: device columns must be contiguous")
-            kind = kind or _torch_kind(values)
-            if kind not in _KIND_BYTES:
-                raise ValueError(f"Source.compact: unsupported device column dtype {values.dtype} (kind={kind})")
-            nbytes = values.numel() * values.element_size()
-            if nbytes % _KIND_BYTES[kind]:
-                raise ValueError("Source.compact: tensor size is not a whole number of entries")
-            return cls(_lib.JB_SOURCE_COMPACT, nbytes // _KIND_BYTES[kind], ptr=values.data_ptr(),
-                       kind=SCALAR_KINDS[kind], on_device=1, keep=values)
-        a, k, n = small_scalars(values, kind)
-        return cls(_lib.JB_SOURCE_COMPACT, n, ptr=a.ctypes.data, kind=k, keep=a)
+        ptr, k, n, dev, keep = _compact_column(values, kind, "Source.compact")
+        return cls(_lib.JB_SOURCE_COMPACT, n, ptr=ptr, kind=k, on_device=dev, keep=keep)
 
     @classmethod
     def one_hot(cls, addresses, K: int, r_addr) -> "Source":
@@ -1123,21 +1111,15 @@ class G1Bases:
         sums the bases[idx mod row_width] of its hot indices. Returns (count, R, 12) Jacobian limbs, R = K T / row_width."""
         if layout not in ONE_HOT_LAYOUTS:
             raise ValueError(f"one_hot_rows: layout must be one of {sorted(ONE_HOT_LAYOUTS)}")
-        if isinstance(columns, np.ndarray) and columns.ndim == 1:
-            columns = [columns]
-        cols = [np.ascontiguousarray(c) for c in columns]
-        if not cols:
+        ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_rows")
+        if not ptrs:
             return np.zeros((0, 0, 12), dtype=np.uint64)
-        dt = cols[0].dtype
-        if dt not in ONE_HOT_NONE or any(c.dtype != dt or c.ndim != 1 or c.shape != cols[0].shape for c in cols):
-            raise ValueError("one_hot_rows: columns must be 1-D uint8 or uint16 arrays of one dtype and length")
-        T = cols[0].shape[0]
+        if dev:
+            raise ValueError("one_hot_rows: columns must be host arrays")
         rows = K * T // row_width if row_width > 0 and K * T >= row_width else 0
-        out = np.zeros((len(cols), max(rows, 1), 12), dtype=np.uint64)
-        ptrs = (ctypes.c_void_p * len(cols))(*[c.ctypes.data for c in cols])
-        kind = SCALAR_KINDS["u8" if dt == np.uint8 else "u16"]
-        self.s.check(self.s.lib.jb_msm_g1_one_hot_rows(self.s.h, self.handle, ptrs, len(cols), kind, T, K, row_width,
-                                                       ONE_HOT_LAYOUTS[layout], _p(out)))
+        out = np.zeros((len(ptrs), max(rows, 1), 12), dtype=np.uint64)
+        self.s.check(self.s.lib.jb_msm_g1_one_hot_rows(self.s.h, self.handle, (ctypes.c_void_p * len(ptrs))(*ptrs),
+                                                       len(ptrs), kind, T, K, row_width, ONE_HOT_LAYOUTS[layout], _p(out)))
         return out[:, :rows]
 
     def batch_add(self, index_sets) -> np.ndarray:

@@ -10,10 +10,9 @@
 // host and binding.
 #include <cuda_runtime.h>
 
-#include "ctx.hpp"
+#include "columns.cuh"
 #include "host_fr.hpp"
 #include "poly_kernels.cuh"
-#include "small_scalar.cuh"
 
 using namespace jb;
 
@@ -69,38 +68,27 @@ __global__ void __launch_bounds__(256) bind_small_kernel(const void* values, siz
     }
 }
 
-int valid_kind(int kind) { return kind >= SK_U8 && kind <= SK_LAST; }
-
-int grid_for(jb_ctx* c, size_t items) {
-    size_t need = (items + 255) / 256;
-    size_t cap = (size_t)c->sm_count * 4;
-    size_t g = need < cap ? need : cap;
-    return g < 1 ? 1 : (int)g;
-}
-
 }  // namespace
 
 extern "C" {
 
 int jb_table_upload_small(jb_ctx* c, const void* values, size_t len, int kind, jb_table* out) {
     if (!c || !values || !out || len == 0) return JB_ERR_INVALID;
-    if (!valid_kind(kind)) return c->fail(JB_ERR_INVALID, "upload_small: unknown scalar kind");
+    if (!compact_kind(kind)) return c->fail(JB_ERR_INVALID, "upload_small: unknown scalar kind");
     int st = jb_table_alloc(c, len, out);
     if (st != JB_OK) return st;
     Guard g(c);
     Table& t = c->tables[*out];
-    void* d_vals = nullptr;
-    const size_t bytes = len * (size_t)small_kind_bytes(kind);
-    st = c->dev_alloc(&d_vals, bytes);
-    if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_vals, values, bytes, cudaMemcpyHostToDevice, c->stream), "upload_small H2D");
+    Columns cols(c);
+    const void* d_vals = nullptr;
+    st = cols.get(values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
     // (the caller's buffer is only borrowed for the call: a pinned source makes the copy truly asynchronous)
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "upload_small sync");
     if (st == JB_OK) {
-        promote_small_kernel<<<grid_for(c, len), 256, 0, c->stream>>>(d_vals, len, kind, t.buf);
+        promote_small_kernel<<<launch_grid(c, len, 256, 4), 256, 0, c->stream>>>(d_vals, len, kind, t.buf);
         c->launches++;
         st = c->check(cudaGetLastError(), "promote_small_kernel launch");
     }
-    c->dev_free(d_vals);
     if (st != JB_OK) {
         c->release(t);
         c->tables.erase(*out);
@@ -110,7 +98,7 @@ int jb_table_upload_small(jb_ctx* c, const void* values, size_t len, int kind, j
 
 int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, const uint64_t r[4], int order, jb_table* out) {
     if (!c || !values || !out || !r) return JB_ERR_INVALID;
-    if (!valid_kind(kind)) return c->fail(JB_ERR_INVALID, "bind_small: unknown scalar kind");
+    if (!compact_kind(kind)) return c->fail(JB_ERR_INVALID, "bind_small: unknown scalar kind");
     if (len < 2 || (len & (len - 1))) return c->fail(JB_ERR_INVALID, "bind_small: table length must be a power of two >= 2");
     if (HostFr::geq_p(r)) return c->fail(JB_ERR_INVALID, "bind_small: challenge limbs not canonical (>= r)");
     if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "bind_small: unknown binding order");
@@ -126,21 +114,19 @@ int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, con
         s.w[2 * i] = (uint32_t)sr.l[i];
         s.w[2 * i + 1] = (uint32_t)(sr.l[i] >> 32);
     }
-    void* d_vals = nullptr;
-    const size_t bytes = len * (size_t)small_kind_bytes(kind);
-    st = c->dev_alloc(&d_vals, bytes);
-    if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_vals, values, bytes, cudaMemcpyHostToDevice, c->stream), "bind_small H2D");
+    Columns cols(c);
+    const void* d_vals = nullptr;
+    st = cols.get(values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
     // (the caller's buffer is only borrowed for the call: a pinned source makes the copy truly asynchronous)
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "bind_small sync");
     if (st == JB_OK) {
         if (order == JB_HIGH_TO_LOW)
-            bind_small_kernel<ORDER_HIGH_TO_LOW><<<grid_for(c, half), 256, 0, c->stream>>>(d_vals, half, kind, s, t.buf);
+            bind_small_kernel<ORDER_HIGH_TO_LOW><<<launch_grid(c, half, 256, 4), 256, 0, c->stream>>>(d_vals, half, kind, s, t.buf);
         else
-            bind_small_kernel<ORDER_LOW_TO_HIGH><<<grid_for(c, half), 256, 0, c->stream>>>(d_vals, half, kind, s, t.buf);
+            bind_small_kernel<ORDER_LOW_TO_HIGH><<<launch_grid(c, half, 256, 4), 256, 0, c->stream>>>(d_vals, half, kind, s, t.buf);
         c->launches++;
         st = c->check(cudaGetLastError(), "bind_small_kernel launch");
     }
-    c->dev_free(d_vals);
     if (st != JB_OK) {
         c->release(t);
         c->tables.erase(*out);

@@ -193,6 +193,15 @@ struct jb_ctx {
     void msm_release();
 };
 
+// Blocks of `block` threads for a grid-stride pass over `items`: one per `block` items, at most one wave of
+// `per_sm` resident blocks on every SM, at least one.
+inline unsigned launch_grid(const jb_ctx* c, size_t items, int block, int per_sm) {
+    size_t need = (items + block - 1) / block;
+    size_t resident = (size_t)c->sm_count * per_sm;
+    size_t grid = need < resident ? need : resident;
+    return grid < 1 ? 1u : (unsigned)grid;
+}
+
 // Serialises a context's entry points (a context = one ProofSession; Rayon threads may call msm concurrently,
 // crates/jolt-hyperkzg/src/scheme.rs:141-145). keep_resident: the caller is the resident round path itself.
 struct CtxGuard {

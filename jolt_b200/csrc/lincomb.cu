@@ -16,15 +16,16 @@
 // A call with count <= LC_GROUP stages its descriptors once per block; a longer one restages each group per tile.
 // Either way there is one pass: P is written once and each term is read once. A term shorter than len is the prefix of
 // the index range and contributes nothing beyond its length. A one-hot term at x reads addr[j] (cycle-major
-// x = j K + k, address-major x = k T + j) and compares it with k; an address >= K that is not the none value raises
-// the call's flag, and the entry point then discards the output. Integer arithmetic only: bit-exact and deterministic.
+// x = j K + k, address-major x = k T + j) and compares it with k; a bad address raises the call's flag, and the entry
+// point then discards the output (columns.cuh decides the column formats and their checks). Integer arithmetic only:
+// bit-exact and deterministic.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <vector>
 
+#include "columns.cuh"
 #include "member.hpp"
-#include "small_scalar.cuh"
 
 using namespace jb;
 using namespace jbi;
@@ -78,9 +79,8 @@ __device__ __forceinline__ void lc_term(uint32_t (&A)[17], const LcTerm& t, size
         const size_t j = t.layout == JB_ONE_HOT_CYCLE_MAJOR ? x >> t.log_k : x & (((size_t)1 << t.log_t) - 1);
         const uint32_t k = t.layout == JB_ONE_HOT_CYCLE_MAJOR ? (uint32_t)(x & ((1u << t.log_k) - 1))
                                                               : (uint32_t)(x >> t.log_t);
-        const bool u8 = t.kind == SK_U8;
-        const uint32_t a = u8 ? (uint32_t)static_cast<const uint8_t*>(t.ptr)[j] : (uint32_t)static_cast<const uint16_t*>(t.ptr)[j];
-        if (a == (u8 ? 0xffu : 0xffffu)) return;  // none
+        const uint32_t a = ld_address(t.ptr, j, (int)t.kind);
+        if (a == NO_ADDRESS) return;
         if (a == k) {
 #pragma unroll
             for (int w = 0; w < 8; ++w) c[w] = t.c[w];
@@ -121,13 +121,6 @@ __global__ void __launch_bounds__(LC_BLOCK, 2)
     }
 }
 
-bool pow2(size_t x) { return x != 0 && (x & (x - 1)) == 0; }
-uint32_t log2_of(size_t x) {
-    uint32_t l = 0;
-    while (x >> (l + 1)) ++l;
-    return l;
-}
-
 // The checks of one term that need no allocation; fills its descriptor except the column pointer of a host column.
 int check_term(jb_ctx* c, const jb_lc_term& in, size_t len, LcTerm& t) {
     std::memset(&t, 0, sizeof t);
@@ -141,12 +134,9 @@ int check_term(jb_ctx* c, const jb_lc_term& in, size_t len, LcTerm& t) {
         t.ptr = tab->buf;
         t.len = tab->len;
     } else if (in.type == JB_LC_COMPACT) {
-        if (in.kind < SK_U8 || in.kind > SK_LAST) return c->fail(JB_ERR_INVALID, "linear_combination: unknown scalar kind");
-        if (in.on_device != 0 && in.on_device != 1) return c->fail(JB_ERR_INVALID, "linear_combination: on_device must be 0 or 1");
+        const int st = check_compact_column(c, "linear_combination", in.kind, in.values, in.on_device);
+        if (st != JB_OK) return st;
         if (!pow2(in.len)) return c->fail(JB_ERR_INVALID, "linear_combination: a compact length is not a power of two");
-        if (!in.values) return c->fail(JB_ERR_INVALID, "linear_combination: null column");
-        if (in.on_device && ((uintptr_t)in.values % (size_t)std::min(8, small_kind_bytes(in.kind))))
-            return c->fail(JB_ERR_INVALID, "linear_combination: misaligned device column");
         t.kind = (uint32_t)in.kind;
         t.len = in.len;
         const HostFr r2{{HostFr::R2[0], HostFr::R2[1], HostFr::R2[2], HostFr::R2[3]}};
@@ -164,17 +154,10 @@ int check_term(jb_ctx* c, const jb_lc_term& in, size_t len, LcTerm& t) {
             t.nc[2 * k + 1] = (uint32_t)(neg[k] >> 32);
         }
     } else if (in.type == JB_LC_ONE_HOT) {
-        if (in.kind != SK_U8 && in.kind != SK_U16)
-            return c->fail(JB_ERR_INVALID, "one-hot: addresses must be JB_SCALAR_U8 or JB_SCALAR_U16");
         if (in.layout != JB_ONE_HOT_CYCLE_MAJOR && in.layout != JB_ONE_HOT_ADDRESS_MAJOR)
             return c->fail(JB_ERR_INVALID, "linear_combination: unknown one-hot layout");
-        if (!pow2(in.len) || !pow2(in.K)) return c->fail(JB_ERR_INVALID, "one-hot: K and T must be powers of two");
-        if (in.on_device != 0 && in.on_device != 1) return c->fail(JB_ERR_INVALID, "linear_combination: on_device must be 0 or 1");
-        if (in.len >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "one-hot: T must be < 2^31");
-        if (in.K > ((size_t)1 << 16)) return c->fail(JB_ERR_UNSUPPORTED, "one-hot: K must be <= 2^16");
-        if (!in.values) return c->fail(JB_ERR_INVALID, "linear_combination: null column");
-        if (in.on_device && ((uintptr_t)in.values % (size_t)small_kind_bytes(in.kind)))
-            return c->fail(JB_ERR_INVALID, "one-hot: misaligned device column");
+        const int st = check_one_hot_columns(c, "linear_combination", in.kind, in.len, in.K, in.on_device, &in.values, 1);
+        if (st != JB_OK) return st;
         t.kind = (uint32_t)in.kind;
         t.layout = (uint32_t)in.layout;
         t.log_k = log2_of(in.K);
@@ -226,16 +209,14 @@ int jb_table_linear_combination(jb_ctx* c, const jb_lc_term* terms, size_t count
                       "linear_combination terms H2D");
     if (st == JB_OK) st = c->check(cudaMemsetAsync(d_bad, 0, sizeof(unsigned int), c->stream), "linear_combination flag");
     if (st == JB_OK) {
-        const size_t tiles = (len + LC_BLOCK - 1) / LC_BLOCK;
-        const unsigned grid = (unsigned)std::min<size_t>(tiles, (size_t)c->sm_count * 8);
-        lincomb_kernel<<<grid, LC_BLOCK, 0, c->stream>>>(d_terms, count, len, t.buf, d_bad);
+        lincomb_kernel<<<launch_grid(c, len, LC_BLOCK, 8), LC_BLOCK, 0, c->stream>>>(d_terms, count, len, t.buf, d_bad);
         c->launches++;
         st = c->check(cudaGetLastError(), "lincomb_kernel launch");
     }
     unsigned int bad = 0;
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, c->stream), "linear_combination flag D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "linear_combination sync");
-    if (st == JB_OK && bad) st = c->fail(JB_ERR_INVALID, "one-hot: an address >= K that is not the none value");
+    if (st == JB_OK && bad) st = fail_bad_address(c);
     c->dev_free(d_terms);
     c->dev_free(d_bad);
     if (st != JB_OK) {

@@ -14,9 +14,9 @@
 #include <string>
 #include <vector>
 
+#include "columns.cuh"
 #include "member.hpp"
 #include "resident.cuh"
-#include "small_scalar.cuh"
 #include "sumcheck_host.hpp"
 
 using namespace jb;
@@ -857,19 +857,12 @@ static int check_source(jb_ctx* c, const jb_source& sr, size_t len, size_t* log_
     }
     if (sr.type != JB_SOURCE_COMPACT && sr.type != JB_SOURCE_ONE_HOT)
         return c->fail(JB_ERR_INVALID, "expr sources: unknown source type");
-    const bool one_hot = sr.type == JB_SOURCE_ONE_HOT;
-    if (one_hot ? (sr.kind != JB_SCALAR_U8 && sr.kind != JB_SCALAR_U16) : (sr.kind < JB_SCALAR_U8 || sr.kind > JB_SCALAR_S128))
-        return c->fail(JB_ERR_INVALID, "expr sources: unknown kind (one-hot: JB_SCALAR_U8 / U16; compact: not JB_SCALAR_FR)");
-    if (!sr.values) return c->fail(JB_ERR_INVALID, "expr sources: null column");
-    if (sr.on_device != 0 && sr.on_device != 1) return c->fail(JB_ERR_INVALID, "expr sources: on_device must be 0 or 1");
-    const size_t align = std::min(8, small_kind_bytes(sr.kind));
-    if (sr.on_device && (uintptr_t)sr.values % align) return c->fail(JB_ERR_INVALID, "expr sources: misaligned device column");
-    if (!one_hot) return JB_OK;
-    if (sr.K == 0 || (sr.K & (sr.K - 1)) || sr.K > ((size_t)1 << 16))
-        return c->fail(JB_ERR_INVALID, "expr sources: K must be a power of two in [1, 2^16]");
-    if (len >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "expr sources: a one-hot column must be shorter than 2^31");
-    *log_k = 0;
-    while (((size_t)1 << *log_k) < sr.K) ++*log_k;
+    if (sr.type == JB_SOURCE_COMPACT) return check_compact_column(c, "expr sources", sr.kind, sr.values, sr.on_device);
+    // (here a K above 2^16 is invalid, not unsupported)
+    if (sr.K > ((size_t)1 << 16)) return c->fail(JB_ERR_INVALID, "expr sources: K must be a power of two in [1, 2^16]");
+    const int st = check_one_hot_columns(c, "expr sources", sr.kind, len, sr.K, sr.on_device, &sr.values, 1);
+    if (st != JB_OK) return st;
+    *log_k = (size_t)log2_of(sr.K);
     if (*log_k && !sr.r_addr) return c->fail(JB_ERR_INVALID, "expr sources: null r_addr");
     for (size_t i = 0; i < *log_k; ++i)
         if (!canonical_fr(sr.r_addr + 4 * i)) return c->fail(JB_ERR_INVALID, "expr sources: r_addr limbs not canonical");
@@ -913,8 +906,7 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
         mem->m = D;
         mem->order = order;
         mem->len = len;
-        mem->rounds = 0;
-        while (((size_t)1 << mem->rounds) < len) ++mem->rounds;
+        mem->rounds = (size_t)log2_of(len);
         make_expr(mem, monomials, nmonomials, nsources, D);
         mem->tables.resize(nsources);
         mem->src.resize(nsources);
@@ -934,7 +926,7 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
             t.cap = len / 2;
             t.len = len;
             if (order == JB_LOW_TO_HIGH && (st = c->ensure_alt(t, std::max<size_t>(len / 4, 1))) != JB_OK) break;
-            st = sources_copy_column(c, sr.values, len * (size_t)small_kind_bytes(sr.kind), sr.on_device, &sc.values);
+            st = copy_column(c, sr.values, len * (size_t)small_kind_bytes(sr.kind), sr.on_device, &sc.values);
             if (st == JB_OK && sr.type == JB_SOURCE_ONE_HOT) st = sources_one_hot_eq(c, sc, len, sr.r_addr, log_k[i], d_flag);
         }
         unsigned int flag = 0;
@@ -942,7 +934,7 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
                                        "expr sources: flag D2H");
         // (the caller's columns are borrowed for the call only)
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "expr sources: creation sync");
-        if (st == JB_OK && flag) st = c->fail(JB_ERR_INVALID, "one-hot: an address >= K that is not the none value");
+        if (st == JB_OK && flag) st = fail_bad_address(c);
         c->dev_free(d_flag);
         if (st != JB_OK) {
             discard_sources(mem);

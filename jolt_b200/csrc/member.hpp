@@ -33,15 +33,6 @@ inline BindScalar make_scalar(const uint64_t r[4], bool* hi4) {
 
 inline bool canonical_fr(const uint64_t r[4]) { return !HostFr::geq_p(r); }
 
-// Blocks of `block` threads for a grid-stride pass over `items`: one per `block` items, at most one wave of
-// `per_sm` resident blocks on every SM, at least one.
-inline unsigned launch_grid(const jb_ctx* c, size_t items, int block, int per_sm) {
-    size_t need = (items + block - 1) / block;
-    size_t resident = (size_t)c->sm_count * per_sm;
-    size_t grid = need < resident ? need : resident;
-    return grid < 1 ? 1u : (unsigned)grid;
-}
-
 // Launches one round of a per-round sumcheck kernel over `pairs` pair indices: `kernel(args..., out)`, whose blocks
 // each leave `values` partial sums in the context's partial buffer for the last block to fold. `kind` and `m` label
 // the timed launch (jb_ctx::timing_begin), `what` names a launch error.
@@ -63,29 +54,6 @@ int launch_round(jb_ctx* c, Kernel kernel, int block, size_t smem, int per_sm, s
 // capi.cu
 int bind_table(jb_ctx* c, Table& t, const uint64_t r[4], int order);  // Polynomial::bind_with_order on one table
 int eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, uint64_t* d_out);
-
-// Columns of a call that reads them in place (mle_eval.cu, lincomb.cu): host columns are copied to device memory
-// allocated for the call and freed with it; device columns are used as they are.
-struct Columns {
-    jb_ctx* c;
-    std::vector<void*> owned;
-    explicit Columns(jb_ctx* ctx) : c(ctx) {}
-    ~Columns() {
-        for (void* p : owned) c->dev_free(p);
-    }
-    int get(const void* src, size_t bytes, int on_device, const void** dst) {
-        if (on_device) {
-            *dst = src;
-            return JB_OK;
-        }
-        void* d = nullptr;
-        int st = c->dev_alloc(&d, bytes);
-        if (st != JB_OK) return st;
-        owned.push_back(d);
-        *dst = d;
-        return c->check(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream), "column H2D");
-    }
-};
 
 // Accumulates the host time spent waiting for a round result (jb_ctx_diag).
 struct WaitAcc {
@@ -170,8 +138,7 @@ int sources_round(jb_ctx* c, const jb_member* mem, bool weighted, const jb::Tabl
 int sources_finish(jb_member* mem, const uint64_t r[4]);
 // Releases the columns and eq tables of the sources (after their bind, or when the member is destroyed).
 void sources_release(jb_member* mem);
-// Member-owned device copy of a column (host or device memory), and the one-hot eq table with the address check.
-int sources_copy_column(jb_ctx* c, const void* values, size_t bytes, int on_device, void** out);
+// The one-hot eq table of a source and the check of its addresses.
 int sources_one_hot_eq(jb_ctx* c, SourceCol& s, size_t len, const uint64_t* r_addr, size_t log_k, unsigned int* d_flag);
 
 // resident.cu ------------------------------------------------------------------------------------------------

@@ -3,6 +3,7 @@
 //   * jb_small_evaluate_batch : compact integer columns (the value of the promoted polynomial F::from(v))
 //   * jb_one_hot_evaluate     : one-hot (RA) polynomials straight from their address columns
 //   * jb_one_hot_pushforward  : G[k] = sum_{j: addr_j = k} eq(r_cycle, j), as resident tables
+// (the column formats, their checks and the address loads are columns.cuh's)
 //
 // One skeleton serves the first three. The point is split into n_hi + n_lo coordinates (n_lo <= 11) and the index
 // x = h L + l (L = 2^n_lo), so eq(point, x) = e_hi[h] e_lo[l] with two small tables built by eq_build; the 2^n eq
@@ -27,8 +28,8 @@
 #include <cstring>
 #include <vector>
 
+#include "columns.cuh"
 #include "member.hpp"
-#include "small_scalar.cuh"
 
 using namespace jb;
 using namespace jbi;
@@ -40,7 +41,7 @@ constexpr int EV_LO_MAX = 11;          // e_lo has at most 2^11 entries
 constexpr int EV_BLOCK = 256;
 constexpr uint32_t OH_SMEM_K = 256;    // one-hot evaluation: eq(r_addr, .) staged in shared memory up to 8 KiB
 constexpr uint32_t PF_SMEM_K = 512;    // pushforward: block-private bins (K x 64 B) in shared memory up to 32 KiB
-constexpr uint32_t NO_KEY = 0xffffffffu;
+constexpr uint32_t NO_KEY = NO_ADDRESS;
 
 struct EvalCol {  // one output of a launch: its source and its lane block
     const void* ptr;
@@ -90,9 +91,8 @@ struct OneHotSrc {
             for (uint32_t i = threadIdx.x; i < 2 * K; i += blockDim.x) s[i] = reinterpret_cast<const uint4*>(eq_addr)[i];
     }
     __device__ __forceinline__ void acc(uint32_t (&A)[17], const Fr& e, const void* p, size_t i, const uint4* s) const {
-        const uint32_t a = KIND == SK_U8 ? (uint32_t)static_cast<const uint8_t*>(p)[i] : (uint32_t)static_cast<const uint16_t*>(p)[i];
-        const uint32_t none = KIND == SK_U8 ? 0xffu : 0xffffu;
-        if (a == none) return;
+        const uint32_t a = ld_address(p, i, KIND);
+        if (a == NO_ADDRESS) return;
         if (a >= K) {
             atomicOr(bad, 1u);
             return;
@@ -170,7 +170,6 @@ __global__ void __launch_bounds__(EV_BLOCK)
     const size_t L = (size_t)1 << n_lo;
     const size_t l = (size_t)blockIdx.x * EV_BLOCK + tid;
     const size_t h0 = (size_t)blockIdx.y * rpb, h1 = min(rows, h0 + rpb);
-    const uint32_t none = KIND == SK_U8 ? 0xffu : 0xffffu;
     const Fr el = l < L ? ld_elem<Fr>(e_lo, l) : Fr::zero();
     for (size_t z = blockIdx.z; z < count; z += gridDim.z) {
         unsigned long long* g_bins = lanes + cols[z].out * K * 8;
@@ -186,15 +185,12 @@ __global__ void __launch_bounds__(EV_BLOCK)
             uint32_t a = NO_KEY;
             Fr w;
             if (l < L) {
-                const size_t j = h * L + l;
-                a = KIND == SK_U8 ? (uint32_t)static_cast<const uint8_t*>(p)[j] : (uint32_t)static_cast<const uint16_t*>(p)[j];
-                if (a == none) {
-                    a = NO_KEY;
-                } else if (a >= K) {
+                a = ld_address(p, h * L + l, KIND);  // the none value is NO_KEY (>= K)
+                if (a < K) {
+                    w = fp_mul(ld_elem<Fr>(e_hi, h), el);
+                } else if (a != NO_KEY) {
                     atomicOr(bad, 1u);
                     a = NO_KEY;
-                } else {
-                    w = fp_mul(ld_elem<Fr>(e_hi, h), el);
                 }
             }
             pf_flush(a != NO_KEY && cur != NO_KEY && a != cur, cur, acc, bins, lane);
@@ -235,13 +231,6 @@ __global__ void __launch_bounds__(EV_BLOCK) bins_to_fr_kernel(const unsigned lon
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-bool pow2(size_t x) { return x != 0 && (x & (x - 1)) == 0; }
-int log2_of(size_t x) {
-    int l = 0;
-    while (x >> (l + 1)) ++l;
-    return l;
-}
-
 int check_point(jb_ctx* c, const uint64_t* point, size_t nvars, const char* what) {
     if (nvars && !point) return c->fail(JB_ERR_INVALID, what);
     for (size_t i = 0; i < nvars; ++i)
@@ -306,7 +295,7 @@ struct EvalPlan {
                           "evaluate lanes D2H");
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "evaluate sync");
         if (st != JB_OK) return st;
-        if ((uint32_t)h[nlanes]) return c->fail(JB_ERR_INVALID, "one-hot: an address >= K that is not the none value");
+        if ((uint32_t)h[nlanes]) return fail_bad_address(c);
         jb_wide_lanes_reduce_host(h.data(), count, out);
         if (plain) {
             const HostFr r2{{HostFr::R2[0], HostFr::R2[1], HostFr::R2[2], HostFr::R2[3]}};
@@ -340,22 +329,6 @@ int launch_small(EvalPlan& p, int kind, size_t first, size_t n) {
         case SK_S64: return launch_eval(p, SmallSrc<SK_S64>{}, first, n);
         default: return launch_eval(p, SmallSrc<SK_S128>{}, first, n);
     }
-}
-
-int check_one_hot(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K, int on_device,
-                  const char* what) {
-    if (kind != SK_U8 && kind != SK_U16) return c->fail(JB_ERR_INVALID, "one-hot: addresses must be JB_SCALAR_U8 or JB_SCALAR_U16");
-    if (!pow2(T) || !pow2(K)) return c->fail(JB_ERR_INVALID, "one-hot: K and T must be powers of two");
-    if (on_device != 0 && on_device != 1) return c->fail(JB_ERR_INVALID, "one-hot: on_device must be 0 or 1");
-    if (T >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "one-hot: T must be < 2^31");
-    if (K > ((size_t)1 << 16)) return c->fail(JB_ERR_UNSUPPORTED, "one-hot: K must be <= 2^16");
-    if (count && !columns) return c->fail(JB_ERR_INVALID, what);
-    for (size_t p = 0; p < count; ++p) {
-        if (!columns[p]) return c->fail(JB_ERR_INVALID, what);
-        if (on_device && ((uintptr_t)columns[p] % (size_t)small_kind_bytes(kind)))
-            return c->fail(JB_ERR_INVALID, "one-hot: misaligned device column");
-    }
-    return JB_OK;
 }
 
 }  // namespace
@@ -394,12 +367,8 @@ int jb_small_evaluate_batch(jb_ctx* c, const void* const* columns, size_t count,
     int st = check_point(c, point, nvars, "small_evaluate: null point");
     if (st != JB_OK) return st;
     if (nvars > 40) return c->fail(JB_ERR_UNSUPPORTED, "small_evaluate: at most 40 variables");
-    for (size_t i = 0; i < count; ++i) {
-        if (kinds[i] < SK_U8 || kinds[i] > SK_LAST) return c->fail(JB_ERR_INVALID, "small_evaluate: unknown scalar kind");
-        if (!columns[i]) return c->fail(JB_ERR_INVALID, "small_evaluate: null column");
-        const size_t align = std::min(8, small_kind_bytes(kinds[i]));
-        if (on_device && ((uintptr_t)columns[i] % align)) return c->fail(JB_ERR_INVALID, "small_evaluate: misaligned device column");
-    }
+    for (size_t i = 0; i < count; ++i)
+        if ((st = check_compact_column(c, "small_evaluate", kinds[i], columns[i], on_device)) != JB_OK) return st;
     if (count == 0) return JB_OK;
     Guard g(c);
     EvalPlan p(c);
@@ -426,7 +395,7 @@ int jb_small_evaluate_batch(jb_ctx* c, const void* const* columns, size_t count,
 int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K, int layout,
                         int on_device, const uint64_t* point, uint64_t* out) {
     if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;
-    int st = check_one_hot(c, columns, count, kind, T, K, on_device, "one_hot_evaluate: null pointer");
+    int st = check_one_hot_columns(c, "one_hot_evaluate", kind, T, K, on_device, columns, count);
     if (st != JB_OK) return st;
     if (layout != JB_ONE_HOT_CYCLE_MAJOR && layout != JB_ONE_HOT_ADDRESS_MAJOR)
         return c->fail(JB_ERR_INVALID, "one_hot_evaluate: unknown layout");
@@ -463,7 +432,7 @@ int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int
 int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K,
                            int on_device, const uint64_t* r_cycle, jb_table* out_tables) {
     if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;
-    int st = check_one_hot(c, columns, count, kind, T, K, on_device, "one_hot_pushforward: null pointer");
+    int st = check_one_hot_columns(c, "one_hot_pushforward", kind, T, K, on_device, columns, count);
     if (st != JB_OK) return st;
     const size_t log_t = (size_t)log2_of(T);
     if (count && !out_tables) return c->fail(JB_ERR_INVALID, "one_hot_pushforward: null pointer");
@@ -492,7 +461,7 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
     unsigned int flag = 0;
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(&flag, p.bad(), 4, cudaMemcpyDeviceToHost, c->stream), "pushforward flag D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "pushforward sync");
-    if (st == JB_OK && flag) st = c->fail(JB_ERR_INVALID, "one-hot: an address >= K that is not the none value");
+    if (st == JB_OK && flag) st = fail_bad_address(c);
     // the tables are created only once the bins are known to be valid
     std::vector<jb_table> made;
     for (size_t i = 0; i < count && st == JB_OK; ++i) {
@@ -503,8 +472,7 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
         const jb_table h = c->next_id++;
         c->tables[h] = t;
         made.push_back(h);
-        const unsigned grid = (unsigned)std::min<size_t>((K + EV_BLOCK - 1) / EV_BLOCK, (size_t)c->sm_count * 8);
-        bins_to_fr_kernel<<<grid, EV_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, t.buf);
+        bins_to_fr_kernel<<<launch_grid(c, K, EV_BLOCK, 8), EV_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, t.buf);
         c->launches++;
         st = c->check(cudaGetLastError(), "bins_to_fr_kernel launch");
     }

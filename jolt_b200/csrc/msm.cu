@@ -24,10 +24,10 @@
 #include <cstring>
 #include <vector>
 
+#include "columns.cuh"
 #include "ctx.hpp"
 #include "ec.cuh"
 #include "msm_affine.cuh"
-#include "small_scalar.cuh"
 
 using namespace jb;
 
@@ -682,9 +682,8 @@ __global__ void __launch_bounds__(256) one_hot_sort_kernel(const void* cols, int
     uint32_t col = 0;
     if (e < n) {
         const size_t at = (p_lo << log_t) + e;  // position in the packed columns
-        const uint64_t a = kind == SK_U8 ? ((const uint8_t*)cols)[at] : ((const uint16_t*)cols)[at];
-        const uint64_t none = kind == SK_U8 ? 0xFFu : 0xFFFFu;
-        if (a != none) {
+        const uint64_t a = ld_address(cols, at, kind);
+        if (a != NO_ADDRESS) {
             if (a >> log_k) {
                 if (!SCATTER) atomicOr(bad, 1u);
             } else {
@@ -1176,7 +1175,7 @@ int one_hot_device(jb_ctx* c, const Srs& srs, const void* const* columns, size_t
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(c->h_small, d_bad, 4, cudaMemcpyDeviceToHost, c->stream), "one_hot_rows flag D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "one_hot_rows sync");
     if (st == JB_OK && *(const unsigned int*)c->h_small)
-        st = c->fail(JB_ERR_INVALID, "one_hot_rows: an address is >= K and not the none value");
+        st = fail_bad_address(c);
     c->dev_free(d_cols);
     c->dev_free(sorted);
     c->dev_free(hist);
@@ -1442,7 +1441,7 @@ int jb_msm_g1(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* scalars, size_
 
 int jb_msm_g1_small(jb_ctx* c, jb_srs h, size_t offset, const void* scalars, size_t n, int kind, uint64_t out_xyz[12]) {
     if (!c || !out_xyz || (n && !scalars)) return JB_ERR_INVALID;
-    if (kind < SK_U8 || kind > SK_LAST) return c->fail(JB_ERR_INVALID, "msm_small: unknown scalar kind");
+    if (!compact_kind(kind)) return c->fail(JB_ERR_INVALID, "msm_small: unknown scalar kind");
     Guard g(c);
     auto it = c->srs.find(h);
     if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
@@ -1493,7 +1492,7 @@ int jb_msm_g1_batch(jb_ctx* c, jb_srs h, size_t count, const void* const* scalar
         if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
         srs_n = it->second.n;
         for (size_t k = 0; k < count; ++k) {
-            if (kinds[k] < SK_FR || kinds[k] > SK_LAST) return c->fail(JB_ERR_INVALID, "batch_msm: unknown scalar kind");
+            if (kinds[k] != SK_FR && !compact_kind(kinds[k])) return c->fail(JB_ERR_INVALID, "batch_msm: unknown scalar kind");
             if (lens[k] > srs_n) return c->fail(JB_ERR_LENGTH, "batch_msm: a column is longer than the base set");
             if (lens[k] && !scalars[k]) return c->fail(JB_ERR_INVALID, "batch_msm: null column");
         }
@@ -1508,7 +1507,7 @@ int jb_msm_g1_batch(jb_ctx* c, jb_srs h, size_t count, const void* const* scalar
 
 int jb_msm_g1_rows(jb_ctx* c, jb_srs h, const void* scalars, size_t rows, size_t row_width, int kind, uint64_t* out_xyz) {
     if (!c || (rows && row_width && (!scalars || !out_xyz)) || (rows && !out_xyz)) return JB_ERR_INVALID;
-    if (kind < SK_FR || kind > SK_LAST) return c->fail(JB_ERR_INVALID, "msm_rows: unknown scalar kind");
+    if (kind != SK_FR && !compact_kind(kind)) return c->fail(JB_ERR_INVALID, "msm_rows: unknown scalar kind");
     if (rows == 0) return JB_OK;
     if (row_width == 0) {
         for (size_t r = 0; r < rows; ++r) identity_xyz(out_xyz + 12 * r);
@@ -1553,12 +1552,6 @@ int jb_msm_g1_rows(jb_ctx* c, jb_srs h, const void* scalars, size_t rows, size_t
 int jb_msm_g1_one_hot_rows(jb_ctx* c, jb_srs h, const void* const* columns, size_t count, int kind, size_t T, size_t K,
                            size_t row_width, int layout, uint64_t* out_xyz) {
     if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
-    auto pow2 = [](size_t x) { return x != 0 && (x & (x - 1)) == 0; };
-    auto log2_of = [](size_t x) {
-        int l = 0;
-        while (x >> (l + 1)) ++l;
-        return l;
-    };
     if (kind != SK_U8 && kind != SK_U16) return c->fail(JB_ERR_INVALID, "one_hot_rows: addresses must be JB_SCALAR_U8 or JB_SCALAR_U16");
     if (layout != JB_ONE_HOT_CYCLE_MAJOR && layout != JB_ONE_HOT_ADDRESS_MAJOR) return c->fail(JB_ERR_INVALID, "one_hot_rows: unknown layout");
     if (!pow2(T) || !pow2(K)) return c->fail(JB_ERR_INVALID, "one_hot_rows: K and T must be powers of two");

@@ -1,8 +1,8 @@
 // The source pass of expression members over sources (jb_member_create_expr_sources): rounds 0 and 1 of a member
 // some of whose tables are still witness columns in their own format -
 //   * COMPACT: primitive integers (small_scalar.cuh), value F::from(v) (promote_small);
-//   * ONE_HOT: an address column, value eq(r_addr, addr[j]) gathered from the source's K-entry eq table (staged in
-//     shared memory for K <= SRC_SMEM_K, read through L2 beyond), 0 for the none value;
+//   * ONE_HOT: an address column (columns.cuh), value eq(r_addr, addr[j]) gathered from the source's K-entry eq table
+//     (staged in shared memory for K <= SRC_SMEM_K, read through L2 beyond), 0 for the none value;
 //   * TABLE: a field table, loaded as expr_round_kernel loads it.
 // Round 0 reads the sources; round 1 reads them again, binds them into the len/2 field tables the member allocated
 // at creation and sweeps the bound pairs. The sweep itself (points, monomials, split-eq weight) is expr_sweep, the
@@ -12,8 +12,8 @@
 
 #include <algorithm>
 
+#include "columns.cuh"
 #include "member.hpp"
-#include "small_scalar.cuh"
 
 using namespace jb;
 using namespace jbi;
@@ -42,10 +42,8 @@ __device__ __forceinline__ Fr src_value(const SourceParams& sp, int j, size_t i,
         const bool neg = ld_small(sp.values[j], i, sp.kind[j], mag);
         return promote_small(mag, neg);
     }
-    const bool u8 = sp.kind[j] == SK_U8;
-    const uint32_t a = u8 ? (uint32_t)static_cast<const uint8_t*>(sp.values[j])[i]
-                          : (uint32_t)static_cast<const uint16_t*>(sp.values[j])[i];
-    if (a == (u8 ? 0xffu : 0xffffu) || a >= sp.K[j]) return Fr::zero();  // none (creation refused other a >= K)
+    const uint32_t a = ld_address(sp.values[j], i, sp.kind[j]);
+    if (a >= sp.K[j]) return Fr::zero();  // none (NO_ADDRESS; creation refused any other a >= K)
     if (sp.smem[j] != SRC_NO_SMEM) {
         const uint4* s = reinterpret_cast<const uint4*>(dsm + sp.smem[j]);
         return elem_from<Fr>(s[2 * a], s[2 * a + 1]);
@@ -152,11 +150,10 @@ __global__ void __launch_bounds__(256) source_bind_kernel(const __grid_constant_
 // Flags an address >= K that is not the none value.
 template <class A>
 __global__ void __launch_bounds__(256) check_addresses_kernel(const A* addr, size_t n, uint32_t K, unsigned int* bad) {
-    const uint32_t none = (uint32_t)(A)~(A)0;
     bool b = false;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t a = addr[i];
-        b |= a != none && a >= K;
+        const uint32_t a = ld_address(addr, i, sizeof(A) == 1 ? SK_U8 : SK_U16);
+        b |= a != NO_ADDRESS && a >= K;
     }
     if (b) atomicOr(bad, 1u);
 }
@@ -238,7 +235,7 @@ int sources_finish(jb_member* mem, const uint64_t r[4]) {
     }
     bool hi4;
     const BindScalar s = make_scalar(r, &hi4);
-    const unsigned grid = (unsigned)std::min<size_t>((half + 255) / 256, (size_t)c->sm_count * 4);
+    const unsigned grid = launch_grid(c, half, 256, 4);
     if (mem->order == JB_LOW_TO_HIGH)
         source_bind_kernel<ORDER_LOW_TO_HIGH><<<grid, 256, 0, c->stream>>>(sp, mem->ntables(), tp, half, s);
     else
@@ -259,19 +256,11 @@ void sources_release(jb_member* mem) {
     mem->src.clear();
 }
 
-int sources_copy_column(jb_ctx* c, const void* values, size_t bytes, int on_device, void** out) {
-    int st = c->dev_alloc(out, bytes);
-    if (st != JB_OK) return st;
-    return c->check(cudaMemcpyAsync(*out, values, bytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
-                                    c->stream),
-                    "expr sources: column copy");
-}
-
 int sources_one_hot_eq(jb_ctx* c, SourceCol& sc, size_t len, const uint64_t* r_addr, size_t log_k, unsigned int* d_flag) {
     int st = c->dev_alloc((void**)&sc.eq, (size_t)sc.K * 32);
     if (st == JB_OK) st = eq_build(c, r_addr, log_k, nullptr, sc.eq);
     if (st != JB_OK) return st;
-    const unsigned grid = (unsigned)std::min<size_t>((len + 255) / 256, (size_t)c->sm_count * 8);
+    const unsigned grid = launch_grid(c, len, 256, 8);
     if (sc.kind == SK_U8)
         check_addresses_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint8_t*>(sc.values), len, sc.K, d_flag);
     else

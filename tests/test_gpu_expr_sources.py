@@ -416,7 +416,9 @@ def _create(sess, srcs, monomials, length, w=None, order=LOW_TO_HIGH):
         arr[i].type, arr[i].kind, arr[i].on_device = s.get("type", 1), s.get("kind", 1), s.get("on_device", 0)
         arr[i].table = s.get("table", 0)
         v = s.get("values")
-        if v is not None:
+        if isinstance(v, int):      # a raw (device) address
+            arr[i].values = v
+        elif v is not None:
             keep.append(v)
             arr[i].values = v.ctypes.data
         arr[i].K = s.get("K", 0)
@@ -463,6 +465,11 @@ def test_errors_and_context_stays_usable(sess):
     assert _create(sess, [dict(one_hot, r_addr=None)], m1, 16) == INV            # a null r_addr
     assert _create(sess, [dict(compact, values=None)], m1, 16) == INV            # a null column
     assert _create(sess, [dict(compact, on_device=2)], m1, 16) == INV            # on_device not 0 / 1
+    import torch
+    dev = torch.zeros(64, dtype=torch.int64, device="cuda")
+    assert _create(sess, [dict(compact, kind=4, values=dev.data_ptr() + 4, on_device=1)], m1, 16) == INV  # misaligned
+    assert _create(sess, [dict(one_hot, kind=2, values=dev.data_ptr() + 1, on_device=1)], m1, 16) == INV  # misaligned
+    assert _create(sess, [one_hot], m1, 1 << 31) == UNS                          # a one-hot column of 2^31 cycles
     assert _create(sess, [compact], m1, 12) == INV                               # len not a power of two
     assert _create(sess, [compact], m1, 1) == INV                                # len < 2
     p = Polynomial.new(sess, rand_limbs(3, 32))

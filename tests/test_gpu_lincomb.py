@@ -195,6 +195,23 @@ def test_host_and_device_columns_agree(sess):
     assert np.array_equal(a, b)
 
 
+@pytest.mark.parametrize("kind", ["u128", "s128"])
+def test_device_records_need_only_8_byte_alignment(sess, kind):
+    """A device column is aligned to min(8, entry bytes): 16- and 24-byte records at base + 8 are read in place."""
+    import torch
+    n, c = 6, coeff(4, 9)
+    vals = compact_values(kind, 1 << n, np.random.default_rng(9))
+    a, _, _ = small_scalars(vals, kind)
+    buf = torch.zeros(a.size + 8, dtype=torch.int64, device="cuda")
+    off = next(o for o in range(1, 8) if (buf.data_ptr() + 8 * o) % 16 and (buf.data_ptr() + 8 * o) % 24)
+    col = buf[off:off + a.size]
+    col.copy_(torch.from_numpy(a.view(np.int64).reshape(-1).copy()))
+    P = Polynomial.linear_combination(sess, [LinearTerm.compact(col, c, kind=kind)])
+    assert P.to_ints() == LR.linear_combination([("compact", SR.decode_column(a, kind), c)], 1 << n)
+    pt = O.random_fr(10, n)
+    assert evaluate_small(sess, col, pt, kinds=kind) == evaluate_small(sess, [vals], pt, kinds=kind)
+
+
 def _scale_terms(sess, n, count, seed, one_hot_K=16):
     t = Terms(sess, seed, big=True)
     kinds = ["u8", "u64", "i128", "i64", "u16", "s64"]

@@ -288,6 +288,14 @@ def test_errors_and_the_context_stays_usable(sess):
     ol = np.zeros((1, 4), dtype=np.uint64)
     assert lib.jb_small_evaluate_batch(h, ptrs, 1, (ctypes.c_int * 1)(0), 16, 0, _p(F.ints_to_limbs(pt)), 4, _p(ol)) == INV
     assert lib.jb_small_evaluate_batch(h, ptrs, 1, (ctypes.c_int * 1)(10), 16, 0, _p(F.ints_to_limbs(pt)), 4, _p(ol)) == INV
+    import torch
+    dev = torch.zeros(64, dtype=torch.int64, device="cuda")
+    u8k, u64k = (ctypes.c_int * 1)(1), (ctypes.c_int * 1)(4)
+    nul = (ctypes.c_void_p * 1)(None)
+    assert lib.jb_small_evaluate_batch(h, ptrs, 1, u8k, 16, 2, _p(F.ints_to_limbs(pt)), 4, _p(ol)) == INV  # on_device
+    assert lib.jb_small_evaluate_batch(h, nul, 1, u8k, 16, 0, _p(F.ints_to_limbs(pt)), 4, _p(ol)) == INV   # null column
+    assert lib.jb_small_evaluate_batch(h, (ctypes.c_void_p * 1)(dev.data_ptr() + 4), 1, u64k, 16, 1,        # misaligned
+                                       _p(F.ints_to_limbs(pt)), 4, _p(ol)) == INV
     addr = np.array([0, 1, 2, 3, 0xFF, 1, 0, 2], dtype=np.uint8)
     opt = point("random", 5, 6)
     with pytest.raises(ValueError):
@@ -299,6 +307,13 @@ def test_errors_and_the_context_stays_usable(sess):
     assert lib.jb_one_hot_evaluate(h, aptrs, 1, 4, 8, 4, 0, 0, _p(o5), _p(ol)) == INV  # u64 addresses
     assert lib.jb_one_hot_evaluate(h, aptrs, 1, 1, 8, 4, 2, 0, _p(o5), _p(ol)) == INV  # unknown layout
     assert lib.jb_one_hot_evaluate(h, aptrs, 1, 1, 1 << 31, 4, 0, 0, _p(o5), _p(ol)) == UNS
+    assert lib.jb_one_hot_evaluate(h, aptrs, 1, 1, 8, 1 << 17, 0, 0, _p(o5), _p(ol)) == UNS   # K > 2^16
+    assert lib.jb_one_hot_evaluate(h, aptrs, 1, 1, 8, 4, 0, 2, _p(o5), _p(ol)) == INV  # on_device
+    assert lib.jb_one_hot_evaluate(h, nul, 1, 1, 8, 4, 0, 0, _p(o5), _p(ol)) == INV    # null column
+    odd = (ctypes.c_void_p * 1)(dev.data_ptr() + 1)
+    assert lib.jb_one_hot_evaluate(h, odd, 1, 2, 8, 4, 0, 1, _p(o5), _p(ol)) == INV    # misaligned u16 device column
+    oh = np.zeros(1, dtype=np.uint64)
+    assert lib.jb_one_hot_pushforward(h, odd, 1, 2, 8, 4, 1, _p(F.ints_to_limbs(opt[:3])), _p(oh)) == INV
     assert lib.jb_one_hot_pushforward(h, aptrs, 1, 1, 8, 4, 0, None, None) == INV
     assert lib.jb_one_hot_evaluate(h, aptrs, 0, 1, 8, 4, 0, 0, _p(o5), _p(ol)) == _lib.JB_OK
     # an address >= K that is not the none value: found on the device

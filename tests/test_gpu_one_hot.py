@@ -217,6 +217,9 @@ def test_errors_then_a_valid_call(sess, srs):
         bases.one_hot_rows(c8, 16, 16, layout="row_major")
     with pytest.raises(ValueError):
         bases.one_hot_rows(c8.astype(np.uint32), 16, 16)
+    import torch
+    with pytest.raises(ValueError, match="one_hot_rows"):   # host columns only
+        bases.one_hot_rows(torch.from_numpy(c8).cuda(), 16, 16)
     # the same context then commits a valid column correctly
     for layout in LAYOUTS:
         got = bases.one_hot_rows(c8, 16, 16, layout)[0]
