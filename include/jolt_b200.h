@@ -238,6 +238,30 @@ typedef struct jb_source {
 int jb_member_create_expr_sources(jb_ctx* ctx, const jb_source* sources, size_t nsources, size_t len,
                                   const jb_monomial* monomials, size_t nmonomials, const uint64_t* eq_w_or_null,
                                   size_t nvars, const uint64_t* eq_scale_or_null, int order, jb_member** out);
+/* Product member over sources: ProveRounds for the product of d = nsources witness polynomials, 1 <= d <= 16,
+ *   sum_x [scale * eq(w, x) *] prod_{i < d} f_i(x),
+ * e.g. the cycle phase of one-hot read checking / RA virtualization with the address split into d chunks,
+ * sum_j eq(r_cycle, j) prod_i ra_i(r_addr_i, j) (the reference's eq-weighted product of many multilinear polynomials,
+ * legacy subprotocols/mles_product_sum.rs), which no sum of smaller members can express. Each f_i is a jb_source with
+ * exactly the semantics, ownership, on-device rules and checks of jb_member_create_expr_sources (table sources owned
+ * by the member, columns copied at creation, everything the rounds need allocated here so JB_ERR_OOM can only arise
+ * here, a bad address found on the device at creation with nothing left allocated).
+ *  - degree = d, + 1 with eq_w_or_null (nvars = log2 len elements, w[0] <-> the most significant index bit, optional
+ *    scale): jb_member_prove_round writes degree + 1 evaluations (up to 18). With eq the running claim is mandatory
+ *    in prove_round, a zero eq factor at the current variable is refused and jb_eq_member_scalar returns
+ *    scale * eq(w, r) after the rounds, as for the other eq members.
+ *  - jb_member_final_evals returns the d bound values in source order.
+ *  - Round polynomials and final evaluations are bit-identical to the direct evaluation of prod_i f_i (and to
+ *    jb_member_create_expr_sources with the single monomial (1, [0 .. d-1]) where d <= 6).
+ *  - jb_prove_batch takes the member at any degree; jb_scheduler_create returns JB_ERR_UNSUPPORTED for a member of
+ *    degree >= 8 (its out_evals stride is 8 elements; jb_prove_batch then proves the rounds in member order).
+ * Errors, before anything is allocated: those of jb_member_create_expr_sources for the same inputs, JB_ERR_INVALID
+ * for nsources == 0, JB_ERR_UNSUPPORTED for nsources > JB_PRODUCT_MAX_FACTORS. The member never runs in a resident
+ * kernel and is not sharded (jb_member_prove_round_partials returns JB_ERR_UNSUPPORTED). */
+#define JB_PRODUCT_MAX_FACTORS 16
+int jb_member_create_product_sources(jb_ctx* ctx, const jb_source* sources, size_t nsources, size_t len,
+                                     const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
+                                     int order, jb_member** out);
 /* Multi-GPU: like prove_round but leaves this rank's partial sums - the kernel values s(0), [s(1) unless
  * skip_t1], s(2), .., s(m-1), s(inf) in the order jb_round_evals_from_kernel_values documents - on the device as
  * count x 8 uint64 lanes, each holding one 32-bit limb (exact under ncclSum over <= 2^32 ranks); the caller

@@ -26,6 +26,7 @@ from .api import (  # noqa: F401
     LinearTerm,
     Polynomial,
     ProductMember,
+    ProductSourcesMember,
     ProvedBatch,
     RoundScheduler,
     Session,

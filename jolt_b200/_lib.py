@@ -60,6 +60,8 @@ SIGNATURES = {
                                              ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_create_expr_sources": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_u64p,
                                                      c_size_t, c_u64p, ctypes.c_int, ctypes.POINTER(c_void_p)]),
+    "jb_member_create_product_sources": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_u64p, c_size_t, c_u64p,
+                                                        ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_prove_round_partials": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, c_void_p]),
     "jb_ctx_set_verify_rounds": (ctypes.c_int, [c_void_p, ctypes.c_int]),
     "jb_partials_finalize": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_u64p]),
@@ -137,6 +139,7 @@ class RoundWorkC(ctypes.Structure):
 
 
 JB_EXPR_MAX_TABLES, JB_EXPR_MAX_MONOMIALS, JB_EXPR_MAX_DEGREE = 8, 16, 6
+JB_PRODUCT_MAX_FACTORS = 16
 
 
 class MonomialC(ctypes.Structure):

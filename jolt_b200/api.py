@@ -505,6 +505,13 @@ class ProductMember:
         self.h = h
         self.m = len(polys)
 
+    @classmethod
+    def from_sources(cls, session: Session, sources: list["Source"], w_limbs=None, scale=None,
+                     order: int = HIGH_TO_LOW) -> "ProductSourcesMember":
+        """The product of up to 16 sources, optionally times a split eq (jb_member_create_product_sources): a
+        ProductSourcesMember (see there)."""
+        return ProductSourcesMember.from_sources(session, sources, w_limbs, scale, order)
+
     def num_rounds(self) -> int:
         n = ctypes.c_size_t()
         self.s.check(self.s.lib.jb_member_num_rounds(self.h, ctypes.byref(n)))
@@ -730,6 +737,47 @@ class ExpressionMember(ProductMember):
             session.h, ctypes.cast(arr, ctypes.c_void_p), len(sources), lens.pop(), ctypes.cast(mons, ctypes.c_void_p),
             len(monomials), _p(w) if w is not None else None, 0 if w is None else w.shape[0],
             _p(sc) if sc is not None else None, order, ctypes.byref(h)))
+        for src in sources:
+            if src.poly is not None:
+                src.poly.handle = 0  # ownership moved into the member
+        self = cls.__new__(cls)
+        self.s = session
+        self.h = h
+        self.ntables = len(sources)
+        d = ctypes.c_size_t()
+        session.check(session.lib.jb_member_degree(h, ctypes.byref(d)))
+        self._degree = d.value
+        self.m = d.value
+        return self
+
+
+class ProductSourcesMember(ExpressionMember):
+    """ProveRounds member for the product of up to 16 sources, optionally times a split eq
+    (jb_member_create_product_sources): sum_x [scale * eq(w, x) *] prod_i f_i(x), degree d (+ 1 with eq) - e.g. the
+    cycle phase of one-hot read checking with the address split into d chunks, sum_j eq(r_cycle, j) prod_i ra_i(j).
+    final_evals() returns one value per source, in order."""
+
+    @classmethod
+    def from_sources(cls, session: Session, sources: list["Source"], w_limbs=None, scale=None,
+                     order: int = HIGH_TO_LOW) -> "ProductSourcesMember":
+        """The product of the sources: each factor is a Source - a device Polynomial, a compact integer column or a
+        one-hot address column, host arrays or CUDA tensors - read as it is until the member's second round binds it.
+        With `w_limbs` (n elements, w[0] <-> MSB) the eq factor is kept split as in EqProductMember and the running
+        claim is mandatory."""
+        lens = {s.length for s in sources}
+        if len(lens) > 1:
+            raise ValueError("from_sources: every source must have one length")
+        arr = (_lib.SourceC * max(len(sources), 1))()
+        keep = []
+        for i, src in enumerate(sources):
+            src._fill(arr[i], keep)
+        w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
+        sc = None if scale is None else _limbs(scale)
+        h = ctypes.c_void_p()
+        session.check(session.lib.jb_member_create_product_sources(
+            session.h, ctypes.cast(arr, ctypes.c_void_p), len(sources), lens.pop() if lens else 0,
+            _p(w) if w is not None else None, 0 if w is None else w.shape[0], _p(sc) if sc is not None else None, order,
+            ctypes.byref(h)))
         for src in sources:
             if src.poly is not None:
                 src.poly.handle = 0  # ownership moved into the member

@@ -11,7 +11,8 @@
 
 #include "../../include/jolt_b200.h"
 
-constexpr int JB_MAX_EVALS = 8;                 // degree + 1 <= 8
+constexpr int JB_MAX_EVALS = 8;                 // degree + 1 <= 8: the scheduler's out_evals stride (ABI)
+constexpr int JB_MAX_ROUND_EVALS = JB_PRODUCT_MAX_FACTORS + 2;  // degree + 1 of any member (a product of 16 times eq)
 constexpr size_t JB_SMALL_BYTES = 4096;         // staging for round evaluations / points
 constexpr int JB_RESULT_SLOTS = 16;             // host-mapped round-result slots (1 KiB each; slot 0 = in-place rounds)
 

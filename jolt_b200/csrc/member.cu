@@ -24,7 +24,8 @@ using namespace jbi;
 using Guard = CtxGuard;
 
 
-// result slots in host-mapped memory: slot s = h_result + s * JB_SLOT_U64: [0, 64) values, [64] sequence flag
+// result slots in host-mapped memory: slot s = h_result + s * JB_SLOT_U64: [0, 64) values, [64] sequence flag, [72, 76)
+// a 17th value (the product pass of 16 factors in verify mode, slot_values)
 constexpr int JB_SLOT_U64 = 128;
 
 namespace {
@@ -226,11 +227,7 @@ int jb_member_num_tables(jb_member* mem, size_t* tables) {
 // lanes_out holds them widened to one 32-bit limb per u64.
 static void* const JB_LANES_EXCHANGE = (void*)(uintptr_t)1;  // sentinel: all-reduce in the kernel epilogue
 
-struct EqRound {
-    const uint64_t* e_out;
-    const uint64_t* e_in;
-    int in_bits;
-};
+using EqRound = EqWeights;
 
 static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* lanes_out, const EqRound* eqr = nullptr,
                         int slot = 0, uint64_t* seq_out = nullptr) {
@@ -254,20 +251,27 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
     const int T = mem->ntables();
     const bool from_src = !mem->src.empty();
     auto is_src = [&](int j) { return from_src && mem->src[j].type != JB_SOURCE_TABLE; };
+    const uint64_t* ins[JB_PRODUCT_MAX_FACTORS];  // (a product member has up to 16 tables, TablePtrs holds 8)
+    uint64_t* outs[JB_PRODUCT_MAX_FACTORS];
     for (int j = 0; j < T; ++j) {
         Table& t = mem->tables[j];
-        tp.in[j] = t.buf;
-        tp.out[j] = t.buf;
+        ins[j] = t.buf;
+        outs[j] = t.buf;
         if (is_src(j)) {  // read from its column; the bind writes the len/2 buffer allocated at creation
-            tp.in[j] = nullptr;
+            ins[j] = nullptr;
             continue;
         }
         if (do_bind && mem->order == JB_LOW_TO_HIGH) {
             int st = c->ensure_alt(t, len);
             if (st != JB_OK) return st;
-            tp.out[j] = t.alt;
+            outs[j] = t.alt;
         }
     }
+    if (!mem->product)
+        for (int j = 0; j < T; ++j) {
+            tp.in[j] = ins[j];
+            tp.out[j] = outs[j];
+        }
     RoundOut ro;
     ro.partial = nullptr;  // set by launch_round
     ro.counter = c->d_counter;
@@ -297,7 +301,9 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
         ro.flag = slot_dev + 64;
     }
     int st;
-    if (eqr) {
+    if (mem->product) {
+        st = product_round(c, mem, ins, outs, eqr, eqr ? true : skip1, pairs, do_bind, hi4, s, ro);
+    } else if (eqr) {
         tp.e_out = eqr->e_out;
         tp.e_in = eqr->e_in;
         tp.in_bits = eqr->in_bits;
@@ -346,15 +352,25 @@ static int resident_values(int D, const uint64_t* lanes, uint64_t* vals);
 static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
 
 struct RoundConsts {
-    HostFr w[6], ipow[6], mpow;
+    HostFr w[JB_PRODUCT_MAX_FACTORS], ipow[JB_PRODUCT_MAX_FACTORS], mpow;
+    HostFr next[JB_PRODUCT_MAX_FACTORS + 1];  // q(M+1) = sum_{i<=M} next_i q(i) for deg q <= M: (-1)^(M-i) C(M+1, i)
 };
-// M in 2..6: products of up to 4 tables; expression members up to degree 6 (jb_round_evals_from_kernel_values stays at 4)
+// M in 1..16: products of up to 16 tables, expression members up to degree 6 (jb_round_evals_from_kernel_values stays
+// at 4). The binomials come from Pascal's triangle (C(17, 8) = 24310 at most).
 static const RoundConsts& round_consts(int M) {
-    static RoundConsts table[7];
+    static RoundConsts table[JB_PRODUCT_MAX_FACTORS + 1];
     static const bool init = [] {
-        static const uint64_t binom[7][7] = {{1}, {1, 1}, {1, 2, 1}, {1, 3, 3, 1}, {1, 4, 6, 4, 1}, {1, 5, 10, 10, 5, 1},
-                                             {1, 6, 15, 20, 15, 6, 1}};
-        for (int m = 2; m <= 6; ++m) {
+        constexpr int N = JB_PRODUCT_MAX_FACTORS + 2;
+        uint64_t binom[N][N] = {{0}};
+        for (int n = 0; n < N; ++n) {
+            binom[n][0] = 1;
+            for (int i = 1; i <= n; ++i) binom[n][i] = binom[n - 1][i - 1] + (i < n ? binom[n - 1][i] : 0);
+        }
+        for (int m = 1; m <= JB_PRODUCT_MAX_FACTORS; ++m) {
+            for (int i = 0; i <= m; ++i) {
+                const HostFr b = HostFr::from_u64(binom[m + 1][i]);
+                table[m].next[i] = ((m - i) & 1) ? HostFr::zero() - b : b;
+            }
             for (int i = 0; i < m; ++i) {
                 HostFr ti = HostFr::one();  // i^m
                 for (int e = 0; e < m; ++e) ti = ti * HostFr::from_u64((uint64_t)i);
@@ -378,7 +394,7 @@ static const RoundConsts& round_consts(int M) {
 // In verify mode the claim is checked (naive.rs:301-308).
 static int assemble_evals(jb_ctx* c, int M, bool skip1, const uint64_t* vals, const uint64_t* claim, size_t round,
                           uint64_t* out_evals) {
-    HostFr ev[JB_MAX_EVALS];
+    HostFr ev[JB_PRODUCT_MAX_FACTORS + 1];
     int k = 0;
     ev[0] = HostFr::from_limbs(vals + 4 * k++);
     if (skip1) ev[1] = HostFr::from_limbs(claim) - ev[0];
@@ -400,6 +416,16 @@ static int assemble_evals(jb_ctx* c, int M, bool skip1, const uint64_t* vals, co
         return c ? c->fail(JB_ERR_ROUND_CHECK, buf) : (int)JB_ERR_ROUND_CHECK;
     }
     return JB_OK;
+}
+
+// The kernel values of a degree-M round in a result slot: the first 16 lie below the slot's sequence flag (word 64),
+// any further ones from word 72 (publish_round's SPLIT); they are copied together into buf when there are more.
+static const uint64_t* slot_values(const uint64_t* slot, int M, bool skip1, uint64_t* buf) {
+    const int k = M == 1 ? (skip1 ? 1 : 2) : (skip1 ? M : M + 1);
+    if (k <= 16) return slot;
+    std::memcpy(buf, slot, 64 * 8);
+    std::memcpy(buf + 64, slot + 72, (size_t)(k - 16) * 32);
+    return buf;
 }
 
 int jb_round_evals_from_kernel_values(int m, int skip_t1, const uint64_t* kernel_values, const uint64_t* claim_or_null,
@@ -594,7 +620,8 @@ int jb_member_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     if (st != JB_OK) return st;
     st = wait_round_result0(c);
     if (st != JB_OK) return st;
-    st = assemble_evals(c, mem->m, skip1, c->h_result, claim, round, out_evals);
+    uint64_t vals[JB_MAX_ROUND_EVALS * 4];
+    st = assemble_evals(c, mem->m, skip1, slot_values(c->h_result, mem->m, skip1, vals), claim, round, out_evals);
     if (st == JB_OK) mem->rounds_done++;
     return st;
 }
@@ -649,28 +676,32 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
     int st = member_round(mem, bind, true, nullptr, &er);
     if (st != JB_OK) return st;
-    // a field inversion is ~400 host multiplications (~13 us): do it while the device runs the pass
+    // a field inversion is ~400 host multiplications (~13 us): do it while the device runs the pass (the
+    // extrapolation constants below are built once)
     const HostFr l1_inv = l1.inverse();
+    const RoundConsts& rc = round_consts((int)M);
     st = wait_round_result0(c);
     if (st != JB_OK) return st;
-    // kernel order: q(0), q(2), .., q(M-1), q(inf)   (M values; q(0) only for M == 1)
+    // kernel order: q(0), q(2), .., q(M-1), q(inf)   (M <= 16 values; q(0) only for M == 1)
     const HostFr q0 = HostFr::from_limbs(c->h_result);
     const HostFr q1 = (HostFr::from_limbs(claim) - l0 * q0) * l1_inv;
-    uint64_t vals[JB_MAX_EVALS * 4], qe[JB_MAX_EVALS * 4];
+    uint64_t vals[JB_MAX_ROUND_EVALS * 4], qe[JB_MAX_ROUND_EVALS * 4];
     q0.store(vals);
     q1.store(vals + 4);
     if (M > 1) std::memcpy(vals + 8, c->h_result + 4, (M - 1) * 32);
     st = assemble_evals(c, (int)M, false, vals, nullptr, round, qe);  // q(0..M)
     if (st != JB_OK) return st;
-    // q(M+1) by extrapolation (degree M), then s(t) = l(t) q(t), t = 0..M+1
-    std::vector<HostFr> qv(M + 1);
-    for (size_t t = 0; t <= M; ++t) qv[t] = HostFr::from_limbs(qe + 4 * t);
-    jb::UnivariatePoly qp = jb::UnivariatePoly::from_evals(qv);
+    // q(M+1) by extrapolation (degree M: the (M+1)-th difference vanishes), then s(t) = l(t) q(t), t = 0..M+1
+    HostFr qv[JB_PRODUCT_MAX_FACTORS + 2];
+    qv[M + 1] = HostFr::zero();
+    for (size_t t = 0; t <= M; ++t) {
+        qv[t] = HostFr::from_limbs(qe + 4 * t);
+        qv[M + 1] = qv[M + 1] + rc.next[t] * qv[t];
+    }
     const HostFr dl = l1 - l0;
     HostFr lt = l0;
     for (size_t t = 0; t <= M + 1; ++t) {
-        HostFr qt = t <= M ? qv[t] : qp.evaluate(HostFr::from_u64(t));
-        (lt * qt).store(out_evals + 4 * t);
+        (lt * qv[t]).store(out_evals + 4 * t);
         lt = lt + dl;
     }
     return JB_OK;
@@ -876,23 +907,25 @@ static void discard_sources(jb_member* mem) {
     delete mem;
 }
 
-int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
-                                  const jb_monomial* monomials, size_t nmonomials, const uint64_t* eq_w_or_null,
-                                  size_t nvars, const uint64_t* eq_scale_or_null, int order, jb_member** out) {
-    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
-    if (!sources || !monomials || !out) return c->fail(JB_ERR_INVALID, "expr sources: null pointer");
+// The creation of a member over sources (expression or product): under the context lock, `check` (the relation's own
+// checks, which return its status first), then the sources, then everything the rounds need is allocated and
+// `shape` makes the new member the relation's member; check sets the member's degree without eq.
+}  // extern "C"
+template <class Check, class Shape>
+static int create_over_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
+                               const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null, int order,
+                               Check check, Shape shape, jb_member** out) {
     jb_member* mem = nullptr;
     int st = JB_OK;
     {
         Guard g(c);
         int D = 0;
-        bool blocks = false;
-        st = check_expr(c, nsources, monomials, nmonomials, eq_w_or_null, nvars, eq_scale_or_null, order, &D, &blocks);
+        st = check(&D);
         if (st != JB_OK) return st;
         if (len < 2 || (len & (len - 1))) return c->fail(JB_ERR_INVALID, "expr sources: len must be a power of two >= 2");
         if (eq_w_or_null && (nvars >= 64 || ((size_t)1 << nvars) != len))
             return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
-        size_t log_k[JB_EXPR_MAX_TABLES] = {0};
+        size_t log_k[JB_PRODUCT_MAX_FACTORS] = {0};
         for (size_t i = 0; i < nsources; ++i) {
             if ((st = check_source(c, sources[i], len, &log_k[i])) != JB_OK) return st;
             for (size_t k = 0; k < i; ++k)
@@ -907,7 +940,7 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
         mem->order = order;
         mem->len = len;
         mem->rounds = (size_t)log2_of(len);
-        make_expr(mem, monomials, nmonomials, nsources, D);
+        shape(mem);
         mem->tables.resize(nsources);
         mem->src.resize(nsources);
         unsigned int* d_flag = nullptr;
@@ -955,6 +988,49 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
     }
     *out = mem;
     return eq_w_or_null ? eq_setup(mem, eq_w_or_null, nvars, eq_scale_or_null, out) : JB_OK;
+}
+extern "C" {
+
+int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
+                                  const jb_monomial* monomials, size_t nmonomials, const uint64_t* eq_w_or_null,
+                                  size_t nvars, const uint64_t* eq_scale_or_null, int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    if (!sources || !monomials || !out) return c->fail(JB_ERR_INVALID, "expr sources: null pointer");
+    int D = 0;
+    auto check = [&](int* D_out) {
+        bool blocks = false;
+        const int st = check_expr(c, nsources, monomials, nmonomials, eq_w_or_null, nvars, eq_scale_or_null, order, &D, &blocks);
+        *D_out = D;
+        return st;
+    };
+    auto shape = [&](jb_member* mem) { make_expr(mem, monomials, nmonomials, nsources, D); };
+    return create_over_sources(c, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null, order, check, shape, out);
+}
+
+// ---- product member over sources ------------------------------------------------------------------------
+int jb_member_create_product_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
+                                     const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
+                                     int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    if (!sources || !out) return c->fail(JB_ERR_INVALID, "product sources: null pointer");
+    // the checks of check_expr that apply to a product, in its order
+    auto check = [&](int* D_out) {
+        if (nsources > JB_PRODUCT_MAX_FACTORS)
+            return c->fail(JB_ERR_UNSUPPORTED, "product sources: at most JB_PRODUCT_MAX_FACTORS sources");
+        if (nsources == 0) return c->fail(JB_ERR_INVALID, "product sources: no sources");
+        if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "product sources: unknown order");
+        if (eq_scale_or_null && !eq_w_or_null) return c->fail(JB_ERR_INVALID, "product sources: a scale without an eq point");
+        if (eq_w_or_null) {
+            for (size_t i = 0; i < nvars; ++i)
+                if (!canonical_fr(eq_w_or_null + 4 * i)) return c->fail(JB_ERR_INVALID, "product sources: point limbs not canonical");
+            if (eq_scale_or_null && !canonical_fr(eq_scale_or_null))
+                return c->fail(JB_ERR_INVALID, "product sources: scale not canonical");
+        }
+        *D_out = (int)nsources;
+        return (int)JB_OK;
+    };
+    auto shape = [&](jb_member* mem) { mem->product = true; };
+    return create_over_sources(c, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null, order, check, shape, out);
 }
 
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
@@ -1125,6 +1201,7 @@ int jb_member_prove_round_partials(jb_member* mem, const uint64_t* bind, size_t 
     if (!mem || !lanes_out) return JB_ERR_INVALID;
     Guard g(mem->ctx, true);
     if (mem->expr) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: expression members are not sharded");
+    if (mem->product) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: product members are not sharded");
     before_launch(mem);
     return member_round(mem, bind, skip_t1 != 0, lanes_out);
 }
@@ -1265,7 +1342,7 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     }
     before_launch(mem);
     if (!mem->src.empty()) {  // len = 2: the sources are bound straight from their columns
-        int st = sources_finish(mem, bind);
+        int st = mem->product ? product_finish(mem, bind) : sources_finish(mem, bind);
         if (st != JB_OK) return st;
     } else {
         for (int j = 0; j < mem->ntables(); ++j) {
@@ -1354,8 +1431,13 @@ int jb_scheduler_create(jb_ctx* c, jb_member** members, size_t n, jb_scheduler**
                 delete s;
                 return c->fail(JB_ERR_INVALID, "scheduler: duplicate member");
             }
+        if (m->m + (m->eq ? 1 : 0) + 1 > JB_MAX_EVALS) {  // out_evals holds JB_MAX_EVALS elements per work item
+            delete s;
+            return c->fail(JB_ERR_UNSUPPORTED, "scheduler: a member of degree >= 8");
+        }
         s->members.push_back(m);
-        if (m->sharded || m->eq || m->expr || members[0]->expr || m->m != members[0]->m || m->terms != members[0]->terms || m->order != members[0]->order)
+        if (m->sharded || m->eq || m->expr || members[0]->expr || m->product || members[0]->product || m->m != members[0]->m ||
+            m->terms != members[0]->terms || m->order != members[0]->order)
             s->homogeneous = false;
     }
     *out = s;
@@ -1521,9 +1603,10 @@ static int overlapped_rounds(jb_scheduler* s, const jb_round_work* work, size_t 
             }
         } else {
             st = wait_round_result(c, (int)i + 1, seqs[i]);
+            uint64_t vals[JB_MAX_ROUND_EVALS * 4];
             if (st == JB_OK)
-                st = assemble_evals(c, m->m, skip[i], c->h_result + (i + 1) * JB_SLOT_U64, w.has_claim ? w.claim : nullptr, w.round,
-                                    out_evals + i * JB_MAX_EVALS * 4);
+                st = assemble_evals(c, m->m, skip[i], slot_values(c->h_result + (i + 1) * JB_SLOT_U64, m->m, skip[i], vals),
+                                    w.has_claim ? w.claim : nullptr, w.round, out_evals + i * JB_MAX_EVALS * 4);
         }
         if (st != JB_OK) return st;
         m->rounds_done++;

@@ -126,8 +126,26 @@ struct jb_member {
     // table j - a compact or one-hot source reads its member-owned column and its Table's buffer is where the bind
     // writes the len/2 field entries. Cleared (and the columns released) by the bind.
     std::vector<SourceCol> src;
+    // product member over sources (jb_member_create_product_sources): the product of its m tables / sources, m <= 16
+    // (terms = 1), through product_round_kernel; src as for the expression member over sources
+    bool product = false;
     int ntables() const { return expr ? ex.ntables : m * terms; }
 };
+
+// The split-eq weight tables of a round (e_out[y >> in_bits] * e_in[y & mask]).
+struct EqWeights {
+    const uint64_t* e_out;
+    const uint64_t* e_in;
+    int in_bits;
+};
+
+// product.cu -------------------------------------------------------------------------------------------------
+// One round of a product member: in / out are the member's m table pointers as member_round prepared them (null in
+// for a source read from its column); eqw: the split-eq weights (then skip1 is set). Rounds 0 and 1 read the sources.
+int product_round(jb_ctx* c, const jb_member* mem, const uint64_t* const* in, uint64_t* const* out, const EqWeights* eqw,
+                  bool skip1, size_t pairs, bool bind, bool hi4, const jb::BindScalar& s, jb::RoundOut ro);
+// The terminal bind of a product member whose sources are still unbound (len = 2).
+int product_finish(jb_member* mem, const uint64_t r[4]);
 
 // sources.cu -------------------------------------------------------------------------------------------------
 // The source pass of rounds 0 (bind == false) and 1 (bind: the sources are bound into their Tables' buffers, field

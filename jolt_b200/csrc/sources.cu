@@ -14,14 +14,13 @@
 
 #include "columns.cuh"
 #include "member.hpp"
+#include "sources.cuh"
 
 using namespace jb;
 using namespace jbi;
 
 namespace {
 
-constexpr uint32_t SRC_SMEM_K = 256;  // a one-hot source's eq table is staged in shared memory up to 8 KiB
-constexpr uint32_t SRC_NO_SMEM = 0xffffffffu;
 // the largest dynamic shared memory of a launch: the columns and block-sum scratch of 8 tables, 8 staged eq tables
 constexpr size_t SRC_SMEM_MAX = expr_smem_bytes(EXPR_MAX_TABLES) + (size_t)EXPR_MAX_TABLES * SRC_SMEM_K * 32;
 
@@ -34,22 +33,6 @@ struct SourceParams {
     uint8_t type[EXPR_MAX_TABLES];        // JB_SOURCE_*
     uint8_t kind[EXPR_MAX_TABLES];
 };
-
-// Entry i of the compact or one-hot source j.
-__device__ __forceinline__ Fr src_value(const SourceParams& sp, int j, size_t i, const uint32_t* dsm) {
-    if (sp.type[j] == JB_SOURCE_COMPACT) {
-        uint32_t mag[4];
-        const bool neg = ld_small(sp.values[j], i, sp.kind[j], mag);
-        return promote_small(mag, neg);
-    }
-    const uint32_t a = ld_address(sp.values[j], i, sp.kind[j]);
-    if (a >= sp.K[j]) return Fr::zero();  // none (NO_ADDRESS; creation refused any other a >= K)
-    if (sp.smem[j] != SRC_NO_SMEM) {
-        const uint4* s = reinterpret_cast<const uint4*>(dsm + sp.smem[j]);
-        return elem_from<Fr>(s[2 * a], s[2 * a + 1]);
-    }
-    return ld_elem<Fr>(sp.eq[j], a);
-}
 
 // expr_round_kernel with step 1 loading each table by its source type (same launch shape, columns and budget).
 // BIND (round 1): a source table is bound from its column into tp.out[j] (the member's len/2 buffer); a field
@@ -133,20 +116,6 @@ __global__ void __launch_bounds__(EXPR_BLOCK, 4)
     round_epilogue<EXPR_MAX_POINTS>(acc, red, out);
 }
 
-// The terminal bind of a member whose sources are unbound: out_j[i] = lo + s (hi - lo) for every compact / one-hot
-// source (the field tables are bound by bind_table).
-template <int ORDER>
-__global__ void __launch_bounds__(256) source_bind_kernel(const __grid_constant__ SourceParams sp, int ntables,
-                                                          const __grid_constant__ TablePtrs tp, size_t half,
-                                                          BindScalar s) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x)
-        for (int j = 0; j < ntables; ++j) {
-            if (sp.type[j] == JB_SOURCE_TABLE) continue;
-            const size_t il = ORDER == ORDER_HIGH_TO_LOW ? i : 2 * i, ih = ORDER == ORDER_HIGH_TO_LOW ? i + half : 2 * i + 1;
-            st_elem(tp.out[j], i, bind_pair<false>(src_value(sp, j, il, nullptr), src_value(sp, j, ih, nullptr), s));
-        }
-}
-
 // Flags an address >= K that is not the none value.
 template <class A>
 __global__ void __launch_bounds__(256) check_addresses_kernel(const A* addr, size_t n, uint32_t K, unsigned int* bad) {
@@ -219,33 +188,11 @@ int sources_round(jb_ctx* c, const jb_member* mem, bool weighted, const TablePtr
 }
 
 int sources_finish(jb_member* mem, const uint64_t r[4]) {
-    jb_ctx* c = mem->ctx;
-    const size_t half = mem->len / 2;
     SourceParams sp;
     fill_params(mem, false, sp);
     TablePtrs tp;
     std::memset(&tp, 0, sizeof tp);
-    for (int j = 0; j < mem->ntables(); ++j) {
-        if (mem->src[j].type == JB_SOURCE_TABLE) {
-            int st = bind_table(c, mem->tables[j], r, mem->order);
-            if (st != JB_OK) return st;
-        } else {
-            tp.out[j] = mem->tables[j].buf;
-        }
-    }
-    bool hi4;
-    const BindScalar s = make_scalar(r, &hi4);
-    const unsigned grid = launch_grid(c, half, 256, 4);
-    if (mem->order == JB_LOW_TO_HIGH)
-        source_bind_kernel<ORDER_LOW_TO_HIGH><<<grid, 256, 0, c->stream>>>(sp, mem->ntables(), tp, half, s);
-    else
-        source_bind_kernel<ORDER_HIGH_TO_LOW><<<grid, 256, 0, c->stream>>>(sp, mem->ntables(), tp, half, s);
-    c->launches++;
-    int st = c->check(cudaGetLastError(), "source_bind_kernel launch");
-    if (st != JB_OK) return st;
-    for (int j = 0; j < mem->ntables(); ++j) mem->tables[j].len = half;
-    sources_release(mem);
-    return JB_OK;
+    return finish_sources(mem, r, sp, tp);
 }
 
 void sources_release(jb_member* mem) {

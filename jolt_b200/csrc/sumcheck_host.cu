@@ -99,8 +99,8 @@ int DeviceProductMember::prove_round(const HostFr* bind, size_t round, const Hos
                                      UnivariatePoly* out) {
     size_t degree = 0;
     jb_member_degree(mem_, &degree);
-    uint64_t ev[8 * 4];  // degree + 1 <= 8 (JB_MAX_EVALS)
-    if (degree + 1 > 8) return JB_ERR_UNSUPPORTED;
+    uint64_t ev[(JB_PRODUCT_MAX_FACTORS + 2) * 4];  // degree <= 17: a product of 16 sources times eq
+    if (degree + 1 > JB_PRODUCT_MAX_FACTORS + 2) return JB_ERR_UNSUPPORTED;
     int st = jb_member_prove_round(mem_, bind ? bind->l : nullptr, round, check_rounds_ ? previous_claim.l : nullptr, ev);
     if (st != JB_OK) return st;
     evals_.resize(degree + 1);
