@@ -80,7 +80,9 @@ class Session:
         ms = (ctypes.c_double * cap)()
         cnt = ctypes.c_size_t()
         self.check(self.lib.jb_ctx_timing_collect(self.h, kinds, items, ms_m, ms, cap, ctypes.byref(cnt)))
-        names = {0: "fused_bind_eval", 1: "bind", 2: "eval_only", 3: "eq", 4: "msm_accumulate"}
+        # resident passes with lookahead sums: 5 binds two variables (items = pairs of the first bind), 6 evaluates (pairs)
+        names = {0: "fused_bind_eval", 1: "bind", 2: "eval_only", 3: "eq", 4: "msm_accumulate", 5: "bind2_eval_look",
+                 6: "eval_look"}
         return [dict(kind=names.get(kinds[i], str(kinds[i])), items=int(items[i]), m=int(ms_m[i]), ms=float(ms[i]))
                 for i in range(cnt.value)]
 

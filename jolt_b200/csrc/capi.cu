@@ -181,6 +181,7 @@ static int ctx_create_impl(int device, bool borrow, void* cuda_stream, jb_ctx** 
     if (const char* ts = std::getenv("JB_RESIDENT_TIMEOUT_S")) c->resident_timeout_cycles = (long long)(std::atof(ts) * 1.9e9);
     if (const char* rs = std::getenv("JB_RES_STAGED")) c->res_staged = std::atoi(rs) != 0;
     if (std::getenv("JB_NO_LOOKAHEAD")) c->lookahead = false;
+    if (const char* fs = std::getenv("JB_RES_FUSE")) c->res_fuse = std::atoi(fs) != 0;
     // A kernel-replaying profiler (ncu) or a serialising tool (compute-sanitizer, nsys CUDA trace) cannot
     // run a kernel that waits for host commands; under CUDA injection keep one launch per round.
     {

@@ -84,6 +84,9 @@ struct jb_ctx {
     bool res_staged = true;         // resident D = 2 products: large passes staged through shared memory (JB_RES_STAGED=0: off)
     long long resident_timeout_cycles = 20000000000LL;  // a resident kernel gives its SMs back after this long without a command
     bool lookahead = true;          // answer thin rounds from the previous answer's lookahead sums (JB_NO_LOOKAHEAD: off)
+    // staged resident runs: answer a large round from the previous pass's lookahead sums and bind its challenge in
+    // the next pass, together with that round's own (JB_RES_FUSE=0: off; needs res_staged and lookahead)
+    bool res_fuse = true;
     std::vector<ResidentRun*> runs; // live resident kernels of this context
     // diagnostics: per round of the last completed run: device %globaltimer at command decode / after the fold,
     // host CLOCK_MONOTONIC at post / at receipt (ns)

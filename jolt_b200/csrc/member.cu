@@ -456,7 +456,8 @@ static void answer_values(const jb_member* mem, const ResConsumed& info, const u
 
 // A thin answer also determines the NEXT round's polynomial as a function of the challenge that round binds.
 static void harvest_lookahead(jb_member* mem, const ResConsumed& info, const uint64_t* lanes) {
-    if ((info.act == RES_ACT_EVAL || info.act == RES_ACT_BIND_EVAL) && info.thin && info.nprime >= 4 && mem->ctx->lookahead) {
+    if ((info.act == RES_ACT_EVAL || info.act == RES_ACT_BIND_EVAL || info.act == RES_ACT_BIND2_EVAL) && info.thin &&
+        info.nprime >= 4 && mem->ctx->lookahead) {
         jb_wide_lanes_reduce_host(lanes, 6, mem->look);
         mem->look_ok = true;
         mem->look_round = info.round + 1;
@@ -486,14 +487,51 @@ struct RunItem {
 // One round of `n` members of one run: ONE mailbox command. Members whose previous answer carried lookahead sums
 // are answered at once from those (their command stays in flight: the device's bind + next sums overlap the
 // caller's Fiat-Shamir step); the others wait for this command's own answer.
+//
+// Large rounds of staged runs are folded (res_fusable): a first round over such tables returns lookahead sums
+// (RES_FLAG_LOOK); the round after it is answered from them with NO command, its challenge left pending on the
+// members; the next command binds the pending challenge and its own in one pass (RES_ACT_BIND2_EVAL) and again
+// returns lookahead sums, so a round after it that is still large is skipped the same way. A round is skipped only
+// when every member of the run takes part, in the same state: then every pending challenge of a run is the same one.
 static int run_round(jb_ctx* c, ResidentRun* run, RunItem* items, int n, const uint64_t* shared_bind, bool exchange,
                      bool gather = false) {
-    unsigned actions[RES_MAX_MEMBERS] = {0};
-    for (int i = 0; i < n; ++i) actions[items[i].mem->run_idx] = items[i].bind ? RES_ACT_BIND_EVAL : RES_ACT_EVAL;
     jb_member* mems[RES_MAX_MEMBERS];
     const int rn = run->n;
     for (int i = 0; i < rn; ++i) mems[i] = run->mem[i];
-    int st = resident_post(run, actions, shared_bind, exchange, gather);
+    const bool fuse = run->fuse && !exchange && !gather;
+    bool skip = fuse && n == rn && resident_inflight(run) == 0, look = fuse;
+    for (int i = 0; i < n; ++i) {
+        const jb_member* m = items[i].mem;
+        if (!items[i].bind) {
+            skip = false;
+            look = look && res_fusable(m->len);
+        } else {
+            skip = skip && !m->pend && m->look_ok && m->look_round == items[i].round && res_fusable(m->len) &&
+                   m->len == items[0].mem->len;
+        }
+    }
+    if (skip) {
+        for (int i = 0; i < n; ++i) {
+            jb_member* m = items[i].mem;
+            uint64_t vals[JB_MAX_EVALS * 4];
+            lookahead_values(m, items[i].bind, vals);
+            m->look_ok = false;
+            m->pend = true;
+            std::memcpy(m->pend_r, items[i].bind, 32);
+            int st = assemble_evals(c, m->m, true, vals, items[i].claim, items[i].round, items[i].out_evals);
+            if (st != JB_OK) return st;
+            m->rounds_done++;
+        }
+        return JB_OK;
+    }
+    unsigned actions[RES_MAX_MEMBERS] = {0};
+    const uint64_t* pending = nullptr;
+    for (int i = 0; i < n; ++i) {
+        jb_member* m = items[i].mem;
+        if (m->pend) pending = m->pend_r;
+        actions[m->run_idx] = !items[i].bind ? RES_ACT_EVAL : m->pend ? RES_ACT_BIND2_EVAL : RES_ACT_BIND_EVAL;
+    }
+    int st = resident_post(run, actions, shared_bind, exchange, gather, pending, look);
     if (st != JB_OK) return st;
     uint64_t out[RES_MAX_MEMBERS * RES_SLOT_U64];
     ResConsumed info[RES_MAX_MEMBERS];
@@ -1335,6 +1373,8 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
         // LowToHigh binds w[var] (the most significant unbound one is w[0]); HighToLow binds w[n - 1 - var]
         eq_absorb_bind(mem, mem->order == JB_LOW_TO_HIGH ? var : mem->eq_n - 1 - var, bind);
     }
+    // right after a round answered from lookahead its challenge is still pending: the run ends (and binds it) first
+    if (mem->run && mem->pend) resident_end(mem->run, false);
     if (mem->run) {
         // the terminal bind is one more mailbox command; a fully bound member gets its values back with the
         // acknowledgement (has_final), so nothing is read from the device afterwards
@@ -1369,7 +1409,7 @@ int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     }
     if (mem->len != 1) {
         char buf[96];
-        size_t remaining = 0;
+        size_t remaining = mem->pend ? (size_t)-1 : 0;  // (a pending challenge is a round already bound)
         for (size_t l = mem->len; l > 1; l >>= 1) ++remaining;
         std::snprintf(buf, sizeof buf, "NotFullyBound { remaining: %zu }", remaining);
         return c->fail(JB_ERR_INVALID, buf);

@@ -118,6 +118,11 @@ struct jb_member {
     bool look_ok = false;
     size_t look_round = 0;
     uint64_t look[6 * 4];
+    // a round answered from lookahead sums with no command: its challenge is bound by the member's next command
+    // (RES_ACT_BIND2_EVAL), or - when the run ends first - by launches as the run is released. len and the tables
+    // do not include it.
+    bool pend = false;
+    uint64_t pend_r[4];
     // expression member (jb_member_create_expr): the summand is ex's weighted monomials over the tables (m = the
     // largest monomial degree, `terms` unused); it never runs in a resident kernel
     bool expr = false;
@@ -186,6 +191,8 @@ struct ResidentRun {
     unsigned grid = 0;
     ResConsumed ring[2][jb::RES_MAX_MEMBERS];  // what command s (slot s & 1) asked of every member
     uint64_t ring_challenge[2][4];             // ... and the challenge it carried (to replay it if the kernel is lost)
+    uint64_t ring_challenge2[2][4];            // ... and the one a RES_ACT_BIND2_EVAL binds first
+    bool fuse = false;                         // staged run: large rounds may be folded into the next pass (res_fusable)
     bool ring_gather[2] = {false, false};      // ... and whether it was a gather (not replayable)
     std::vector<Table> deferred;               // shard buffers a gather made obsolete: freed when the run ends
     struct RoundInfo { int kind; uint64_t items; int m; };
@@ -203,7 +210,10 @@ struct ResidentRun {
 // pointer is dead after that: check mem->run). round = drain + post + consume.
 // gather (single-member run of an index-sharded member, action BIND_EVAL): bind, scatter the bound shard into every
 // rank's arena and sweep the gathered tables; afterwards the member's tables ARE its arena views (len x world).
-int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* challenge, bool exchange, bool gather = false);
+// RES_ACT_BIND2_EVAL binds challenge2 (the member's pending challenge, cleared here), then challenge; `look` sets
+// RES_FLAG_LOOK (the command's EVAL actions are large passes that return lookahead sums).
+int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* challenge, bool exchange, bool gather = false,
+                  const uint64_t* challenge2 = nullptr, bool look = false);
 bool resident_gather_fits(const jb_ctx* c, const jb_member* mem, uint64_t shard_len_after_bind);
 int resident_consume(ResidentRun* run, uint64_t* out, ResConsumed* info);
 int resident_inflight(const ResidentRun* run);

@@ -143,6 +143,15 @@ void release_run(ResidentRun* run, bool mark_no_resident) {
     // later work on the context's stream is ordered after the kernel's exit
     cudaEventRecord(run->res.event, run->res.stream);
     cudaStreamWaitEvent(c->stream, run->res.event, 0);
+    // rounds answered from lookahead whose challenge no command has carried yet: bind it before anything reads the tables
+    for (int i = 0; i < run->n; ++i) {
+        jb_member* m = run->mem[i];
+        if (!m || !m->pend) continue;
+        for (auto& t : m->tables)
+            if (bind_table(c, t, m->pend_r, m->order) != JB_OK) break;  // (the context keeps the error)
+        m->len /= 2;
+        m->pend = false;
+    }
     for (auto& t : run->deferred) c->release(t);
     c->tail_pool.push_back(run->res);
     for (int i = 0; i < run->n; ++i) {
@@ -213,6 +222,7 @@ int resident_begin(jb_ctx* c, jb_member** mems, int n, uint64_t first_len, bool 
     run->n = n;
     run->grid = grid;
     run->exclusive = exclusive;
+    run->fuse = staged && c->res_fuse && c->lookahead;
     int st = acquire_resources(c, &run->res);
     if (st != JB_OK) {
         delete run;
@@ -276,10 +286,15 @@ bool resident_gather_fits(const jb_ctx* c, const jb_member* mem, uint64_t np) {
     return c->xch_ready && c->world <= 16 && (uint64_t)mem->ntables() * (glen + glen / 2) * 32 <= XCH_ARENA_HALF;
 }
 
-int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* challenge, bool exchange, bool gather) {
+int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* challenge, bool exchange, bool gather,
+                  const uint64_t* challenge2, bool look) {
     jb_ctx* c = run->c;
     if (!run->kernel_live) return c->fail(JB_ERR_INVALID, "resident run is not live");
     if (run->seq - run->consumed >= 2) return c->fail(JB_ERR_INVALID, "resident run: two commands already in flight");
+    for (int i = 0; i < run->n; ++i)
+        if ((actions[i] & 0xf) == RES_ACT_BIND2_EVAL &&
+            (exchange || gather || !run->fuse || !challenge2 || !run->mem[i]->pend || std::memcmp(run->mem[i]->pend_r, challenge2, 32) != 0))
+            return c->fail(JB_ERR_INVALID, "resident run: a double bind carries the member's pending challenge");
     const uint64_t seq = run->seq + 1;
     ResMailbox* mb = run->mb;
     ResCmdLine* line = &mb->cmd[seq & 1];
@@ -324,16 +339,28 @@ int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* cha
             ri.m = T;
             continue;
         }
-        slot[i].nprime = a == RES_ACT_BIND_EVAL ? m->len / 2 : m->len;
-        slot[i].thin = (a == RES_ACT_EVAL || a == RES_ACT_BIND_EVAL) && res_is_thin(m->m, slot[i].nprime);
-        if (a == RES_ACT_EVAL || a == RES_ACT_BIND_EVAL) {
-            ri.kind = (a == RES_ACT_BIND_EVAL || ri.kind == 0) ? 0 : 2;
-            ri.items += slot[i].nprime / 2;
+        if (a == RES_ACT_BIND2_EVAL) {
+            cmd |= RES_FLAG_CHALLENGE2;
+            m->pend = false;
+            slot[i].nprime = m->len / 4;
+            slot[i].thin = true;
+            ri.kind = 5;
+            ri.items += m->len / 2;
             ri.m = m->ntables();
+        } else {
+            const bool look_pass = look && a == RES_ACT_EVAL;
+            if (look_pass) cmd |= RES_FLAG_LOOK;
+            slot[i].nprime = a == RES_ACT_BIND_EVAL ? m->len / 2 : m->len;
+            slot[i].thin = (a == RES_ACT_EVAL || a == RES_ACT_BIND_EVAL) && (look_pass || res_is_thin(m->m, slot[i].nprime));
+            if (a == RES_ACT_EVAL || a == RES_ACT_BIND_EVAL) {
+                if (ri.kind != 5) ri.kind = look_pass ? 6 : (a == RES_ACT_BIND_EVAL || ri.kind == 0) ? 0 : 2;
+                ri.items += slot[i].nprime / 2;
+                ri.m = m->ntables();
+            }
         }
         // the host's view of the tables follows the command stream: the device executes commands in order
-        if (a == RES_ACT_BIND_EVAL || a == RES_ACT_FINAL) {
-            m->len /= 2;
+        if (a == RES_ACT_BIND_EVAL || a == RES_ACT_FINAL || a == RES_ACT_BIND2_EVAL) {
+            m->len /= a == RES_ACT_BIND2_EVAL ? 4 : 2;
             for (auto& t : m->tables) {
                 if (m->order == JB_LOW_TO_HIGH) t.swap_buffers();
                 t.len = m->len;
@@ -344,6 +371,10 @@ int resident_post(ResidentRun* run, const unsigned* actions, const uint64_t* cha
     if (challenge) {
         std::memcpy((void*)line->challenge, challenge, 32);
         std::memcpy(run->ring_challenge[seq & 1], challenge, 32);
+    }
+    if (cmd & RES_FLAG_CHALLENGE2) {  // (before cmd_seq below: the device reads it once it has seen the sequence number)
+        std::memcpy((void*)mb->challenge2[seq & 1], challenge2, 32);
+        std::memcpy(run->ring_challenge2[seq & 1], challenge2, 32);
     }
     run->seq = seq;
     if (seq <= 64) {
@@ -403,9 +434,9 @@ int resident_recover(ResidentRun* run) {
     for (uint64_t q = last; q >= first; --q) {
         const ResConsumed* slot = run->ring[q & 1];
         for (int i = 0; i < run->n; ++i) {
-            if (slot[i].act != RES_ACT_BIND_EVAL && slot[i].act != RES_ACT_FINAL) continue;
+            if (slot[i].act != RES_ACT_BIND_EVAL && slot[i].act != RES_ACT_FINAL && slot[i].act != RES_ACT_BIND2_EVAL) continue;
             jb_member* m = run->mem[i];
-            m->len *= 2;
+            m->len *= slot[i].act == RES_ACT_BIND2_EVAL ? 4 : 2;
             for (auto& t : m->tables) {
                 if (m->order == JB_LOW_TO_HIGH) t.swap_buffers();
                 t.len = m->len;
@@ -419,15 +450,18 @@ int resident_recover(ResidentRun* run) {
     for (uint64_t q = first; q <= last && st == JB_OK; ++q) {
         const ResConsumed* slot = run->ring[q & 1];
         for (int i = 0; i < run->n && st == JB_OK; ++i) {
-            if (slot[i].act != RES_ACT_BIND_EVAL && slot[i].act != RES_ACT_FINAL) continue;
+            const unsigned act = slot[i].act;
+            if (act != RES_ACT_BIND_EVAL && act != RES_ACT_FINAL && act != RES_ACT_BIND2_EVAL) continue;
             jb_member* m = run->mem[i];
             for (auto& t : m->tables) {
-                st = bind_table(c, t, run->ring_challenge[q & 1], m->order);
+                if (act == RES_ACT_BIND2_EVAL) st = bind_table(c, t, run->ring_challenge2[q & 1], m->order);
+                if (st == JB_OK) st = bind_table(c, t, run->ring_challenge[q & 1], m->order);
                 if (st != JB_OK) break;
             }
-            if (st == JB_OK) m->len /= 2;
+            if (st == JB_OK) m->len /= act == RES_ACT_BIND2_EVAL ? 4 : 2;
         }
     }
+    // (a member's pending challenge, carried by no command yet, is bound by release_run after these)
     for (int i = 0; i < run->n; ++i) run->mem[i]->look_ok = false;
     run->consumed = run->seq;
     release_run(run, true);

@@ -50,12 +50,18 @@ constexpr int RES_SLOT_U64 = 136;
 constexpr int RES_STATIC_PCT = 75;
 
 // per-member action of a round command (4 bits each, member i at bits [16 + 4i, 20 + 4i) of cmd)
-enum : unsigned { RES_ACT_NONE = 0, RES_ACT_EVAL = 1, RES_ACT_BIND_EVAL = 2, RES_ACT_FINAL = 3 };
+// RES_ACT_BIND2_EVAL (staged kernels): bind by the command's second challenge (the member's pending one), then by its
+// challenge, sweep with lookahead (staged_look_pass) - the tables shrink to a quarter
+enum : unsigned { RES_ACT_NONE = 0, RES_ACT_EVAL = 1, RES_ACT_BIND_EVAL = 2, RES_ACT_FINAL = 3, RES_ACT_BIND2_EVAL = 4 };
 enum : uint64_t { RES_OP_ROUND = 1, RES_OP_ABORT = 2 };
 constexpr uint64_t RES_FLAG_EXCHANGE = 1ull << 8;  // member 0's sums are all-reduced over peer memory
 // member 0 (index-sharded): bind, then write the bound shard into EVERY rank's gather arena, wait for the peers'
 // shards, and sweep the GATHERED tables (G x the shard) - the member continues un-sharded, in the same kernel
 constexpr uint64_t RES_FLAG_GATHER = 1ull << 9;
+// the EVAL actions of this command are large staged passes that also return the lookahead sums (staged_look_pass)
+constexpr uint64_t RES_FLAG_LOOK = 1ull << 10;
+// the command carries a second challenge (ResMailbox::challenge2): some member's action is RES_ACT_BIND2_EVAL
+constexpr uint64_t RES_FLAG_CHALLENGE2 = 1ull << 11;
 
 // The mailbox is a ring of TWO commands / answers (command s uses slot s & 1): with lookahead the host posts
 // command s + 1 while the answer to command s is still on its way.
@@ -85,13 +91,17 @@ struct alignas(64) ResMailbox {
     // finer stamps of the same rounds (diagnostics): [4 s + 0] block 0 finished its passes, [4 s + 1] block 0 arrived
     // on the ticket, [4 s + 2] the last block saw that it is last, [4 s + 3] spare
     uint64_t tlog2[4 * 64];
+    // the second challenge of command s (RES_FLAG_CHALLENGE2), at [s & 1]: written before the line's cmd_seq, read
+    // by the device after it has seen that sequence number (behind a fence)
+    uint64_t challenge2[2][4];
 };
 
 // Device-side re-publication of the command line, the arrival counter and the round's lane accumulators.
 struct alignas(128) ResState {
     uint64_t seq;
     uint64_t cmd[7];
-    uint64_t pad[8];
+    uint64_t challenge2[4];  // (published with cmd)
+    uint64_t pad[4];
     unsigned int ticket;
     unsigned int pad2[31];
     // sequence number of the last round whose sums have been collected (lanes zeroed, ticket reset). With two
@@ -214,6 +224,37 @@ __device__ __noinline__ void resident_pass(const TablePtrs tp, size_t pairs, con
 // bind + sums for round k + 1 overlap the host's Fiat-Shamir step of round k (the answers trail one command behind).
 // Each warp's 17-word accumulator stays in registers and is summed over the warp with two REDUX per word.
 // n' == 2 (the last round): a and b only; c = d = 0, S6 = S7 = 0.
+//
+// Operand of product p (S_p above) for one table of a quad; rd(pos) reads the quad's value at position pos (a b c d).
+template <typename Rd>
+__device__ __forceinline__ Fr look_operand(int p, Rd rd) {
+    switch (p) {  // warp-uniform
+        case 0: return rd(0);
+        case 1: return rd(1);
+        case 2: return fp_sub_lazy(rd(1), rd(0));
+        case 3: return fp_sub_lazy(rd(2), rd(0));
+        case 4: return fp_sub_lazy(rd(3), rd(1));
+        case 5: return fp_sub_lazy(fp_sub(rd(3), rd(2)), fp_sub(rd(1), rd(0)));
+        case 6: return rd(2);
+        default: return fp_sub_lazy(rd(3), rd(2));
+    }
+}
+
+// Warp p's accumulator of product p, summed over the warp (16-bit halves: no overflow in REDUX), into lanes p x 17.
+__device__ __forceinline__ void look_lanes_out(const uint32_t (&A)[17], int p, int g, uint64_t* g_lanes, uint64_t* s_dst) {
+    uint64_t mine = 0;
+#pragma unroll
+    for (int w = 0; w < 17; ++w) {
+        const uint32_t lo = __reduce_add_sync(0xffffffffu, A[w] & 0xffffu);
+        const uint32_t hi = __reduce_add_sync(0xffffffffu, A[w] >> 16);
+        if (g == w) mine = (uint64_t)lo + ((uint64_t)hi << 16);
+    }
+    if (g < 17) {
+        if (s_dst) s_dst[p * 17 + g] = mine;
+        else atomicAdd(reinterpret_cast<unsigned long long*>(g_lanes) + p * 17 + g, (unsigned long long)mine);
+    }
+}
+
 template <int P, int ORDER, bool BIND>
 __device__ __noinline__ void thin_pass(const TablePtrs tp, uint64_t nprime, const BindScalar sc, bool hi4, uint32_t* dsm,
                                        unsigned b, unsigned nblk, uint64_t* g_lanes, uint64_t* s_dst) {
@@ -255,39 +296,18 @@ __device__ __noinline__ void thin_pass(const TablePtrs tp, uint64_t nprime, cons
 #pragma unroll
             for (int jj = 0; jj < 2; ++jj) {
                 const uint32_t* sv = sval + jj * 4 * 8 * 32 + g;
-                auto rd = [&](int ps) {
+                x[jj] = look_operand(p, [&](int ps) {
                     Fr r;
 #pragma unroll
                     for (int w = 0; w < 8; ++w) r.v[w] = sv[(ps * 8 + w) * 32];
                     return r;
-                };
-                switch (p) {  // warp-uniform
-                    case 0: x[jj] = rd(0); break;
-                    case 1: x[jj] = rd(1); break;
-                    case 2: x[jj] = fp_sub_lazy(rd(1), rd(0)); break;
-                    case 3: x[jj] = fp_sub_lazy(rd(2), rd(0)); break;
-                    case 4: x[jj] = fp_sub_lazy(rd(3), rd(1)); break;
-                    case 5: x[jj] = fp_sub_lazy(fp_sub(rd(3), rd(2)), fp_sub(rd(1), rd(0))); break;
-                    case 6: x[jj] = rd(2); break;
-                    default: x[jj] = fp_sub_lazy(rd(3), rd(2)); break;
-                }
+                });
             }
             mul_wide_acc_reg(A, x[0].v, x[1].v);
         }
         __syncthreads();
     }
-    // warp p holds product p: sum each accumulator word over the 32 lanes (16-bit halves: no overflow in REDUX)
-    uint64_t mine = 0;
-#pragma unroll
-    for (int w = 0; w < 17; ++w) {
-        const uint32_t lo = __reduce_add_sync(0xffffffffu, A[w] & 0xffffu);
-        const uint32_t hi = __reduce_add_sync(0xffffffffu, A[w] >> 16);
-        if (g == w) mine = (uint64_t)lo + ((uint64_t)hi << 16);
-    }
-    if (g < 17) {
-        if (s_dst) s_dst[p * 17 + g] = mine;
-        else atomicAdd(reinterpret_cast<unsigned long long*>(g_lanes) + p * 17 + g, (unsigned long long)mine);
-    }
+    look_lanes_out(A, p, g, g_lanes, s_dst);  // warp p holds product p
 }
 
 // ---- staged pass (D = 2, P = 1, more than RES_THIN_PAIRS pairs) ------------------------------------------------
@@ -311,7 +331,10 @@ constexpr int STG_STAGES = 2;
 constexpr uint32_t STG_STAGE_BYTES = 2 * (STG_TILE * 4 * 32 + 128);  // two tables x 4 elements per pair + the offsets
 constexpr uint32_t STG_BAR_OFF = STG_STAGES * STG_STAGE_BYTES;        // mbarriers [STG_STAGES], then tile ids
 constexpr uint32_t STG_RED_OFF = STG_BAR_OFF + STG_STAGES * 16;      // per-warp column sums [8 warps][2 x 17]
-constexpr uint32_t STG_SMEM_BYTES = STG_RED_OFF + (RES_BLOCK / 32) * 2 * 17 * 8;
+constexpr uint32_t STG_XCH_OFF = STG_RED_OFF + (RES_BLOCK / 32) * 2 * 17 * 8;  // staged_look_pass: [8 values][8 words][32 quads]
+constexpr uint32_t STG_SC_OFF = STG_XCH_OFF + 8 * 8 * 32 * 4;                  // ... its two bind scalars
+constexpr uint32_t STG_PROD_OFF = STG_SC_OFF + 2 * 32;                          // ... and its producer's next tile, step, static end
+constexpr uint32_t STG_SMEM_BYTES = STG_PROD_OFF + 16;
 constexpr uint32_t STG_NONE = 0xffffffffu;
 // The cooperative grid is sm_count x (blocks per SM from the occupancy query): a shared-memory budget that allowed
 // only one block per SM would halve it without any error. Static part: a bound on the __shared__ arrays of
@@ -477,6 +500,205 @@ __device__ __noinline__ void staged_pass(const TablePtrs tp, size_t pairs, const
     }
 }
 
+// ---- staged lookahead passes (D = 2, P = 1, tables of more than 4 RES_THIN_PAIRS entries) -----------------------
+// Both return thin_pass's eight sums S0..S7 over the quads of the tables they leave. The host answers the next round
+// from S0..S5 without any device pass and hands that round's challenge to the following pass, which binds two
+// variables in one read of the tables (res_fusable below decides when).
+//   BIND2 = false: eval over T (n entries per table). A tile is 128 quads = 512 entries per table in staged_pass's
+//     bind layout with pairs = n / 4 - its "pair" y is quad y (LowToHigh e0..e3 = a b c d; HighToLow e0 = a,
+//     e1 = c, e2 = b, e3 = d). Warp p accumulates product p of four quads per lane, read straight from the stage.
+//   BIND2 = true: T (n) -> bind sa -> bind sb -> T2 (n / 4, stored) and the sums over T2's quads. A tile is 128 T2
+//     entries per table, 512 T entries, in the same stage layout (LowToHigh: T2[y] <- T[4y .. 4y + 3];
+//     HighToLow: T2[y] <- T[y + u n / 4], u < 4). Under HighToLow a quad of T2 is (T2[q], T2[q + n/8], T2[q + n/16],
+//     T2[q + 3n/16]), so a tile holds the T2 runs q0 + k n/16 + (0 .. 31), k < 4: 16 copies of 1 KiB per table.
+//     Each thread binds one T2 entry (three binds), stores it (HighToLow in place: T[y], y < n / 4, is read only by
+//     the thread that writes T2[y], out of the stage) and puts it into the exchange buffer, from which warp p
+//     accumulates product p of one of the tile's 32 quads per lane - thin_pass's exchange, served from the stage.
+template <int ORDER, bool BIND2>
+__device__ __noinline__ void staged_look_pass(const TablePtrs tp, uint64_t n, const BindScalar sa, const BindScalar sb, bool hi4a,
+                                              bool hi4b, uint8_t* smem, unsigned b, unsigned nblk, uint32_t static_end,
+                                              uint64_t* g_lanes, uint64_t* s_dst) {
+    constexpr uint32_t SUB = 32 * 4 * 32;
+    constexpr uint32_t TOFF = ORDER == ORDER_LOW_TO_HIGH ? 4 * SUB + 64 : 4 * STG_TILE * 32 + 16;
+    constexpr uint32_t ESTEP = ORDER == ORDER_LOW_TO_HIGH ? 32 : STG_TILE * 32;
+    static_assert(2 * TOFF <= STG_STAGE_BYTES, "a tile overflows its stage");
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, j = tid & 1;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + STG_BAR_OFF);
+    uint32_t* tile_id = reinterpret_cast<uint32_t*>(bar + STG_STAGES);
+    const uint64_t quarter = n / 4;
+    const uint32_t ntiles = (uint32_t)(quarter / STG_TILE);
+    const uint32_t xch = smem_u32(smem + STG_XCH_OFF), scs = smem_u32(smem + STG_SC_OFF);
+    // BIND2: this thread's T2 entry of a tile (table j), its quad g and position pos there, and its stage offset
+    int ty, g, pos;
+    uint32_t off;
+    if (ORDER == ORDER_LOW_TO_HIGH) {
+        const int q = (tid >> 1) & 3, r = tid >> 3;
+        ty = q * 32 + r;
+        g = ty >> 2;
+        pos = ty & 3;
+        off = j * TOFF + q * (SUB + 16) + r * 4 * 32;
+    } else {
+        const int pp = tid >> 1, k = pp >> 5;
+        ty = pp;
+        g = pp & 31;
+        pos = ((k & 1) << 1) | (k >> 1);  // runs at q, q + n/16, q + n/8, q + 3n/16 hold a, c, b, d
+        off = j * TOFF + pp * 32;
+    }
+
+    // thread 0's producer state lives in shared memory (next tile, step, static end): the tile loop needs every register
+    const uint32_t prod = smem_u32(smem + STG_PROD_OFF);
+    bool dyn = false, done = false;
+    const auto produce = [&](int s) {
+        uint32_t t = STG_NONE;
+        if (!done) {
+            uint32_t next, step, send;
+            asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(next), "=r"(step) : "r"(prod));
+            asm volatile("ld.shared.u32 %0, [%1+8];" : "=r"(send) : "r"(prod));
+            if (!dyn && next < send) {
+                t = next;
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(prod), "r"(next + step) : "memory");
+            } else {
+                dyn = true;
+                if (send < ntiles) {
+                    const uint32_t c = send + atomicAdd(tp.work, 1u);
+                    if (c < ntiles) t = c;
+                }
+            }
+            done = t == STG_NONE;
+        }
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_u32(tile_id + s)), "r"(t) : "memory");
+        if (t == STG_NONE) {
+            mbar_arrive(&bar[s]);
+            return;
+        }
+        mbar_expect_tx(&bar[s], 2 * STG_TILE * 4 * 32);
+        uint8_t* dst = smem + s * STG_STAGE_BYTES;
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(tp.in[jj]);
+            if (ORDER == ORDER_LOW_TO_HIGH) {
+                const size_t y0 = (size_t)t * STG_TILE;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) bulk_g2s(dst + jj * TOFF + q * (SUB + 16), src + (y0 + 32 * q) * 4 * 32, SUB, &bar[s]);
+            } else if (!BIND2) {
+                const size_t y0 = (size_t)t * STG_TILE;
+#pragma unroll
+                for (int u = 0; u < 4; ++u) bulk_g2s(dst + jj * TOFF + u * STG_TILE * 32, src + (y0 + u * quarter) * 32, STG_TILE * 32, &bar[s]);
+            } else {
+                const size_t q0 = (size_t)t * 32;
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        bulk_g2s(dst + jj * TOFF + u * STG_TILE * 32 + k * 32 * 32, src + (q0 + k * (n / 16) + u * quarter) * 32, 32 * 32,
+                                 &bar[s]);
+            }
+        }
+    };
+
+    if (BIND2 && tid < 16) {  // the scalars wait in shared memory: 16 registers fewer across the tile loop
+        const uint32_t w = tid < 8 ? sa.w[tid & 7] : sb.w[tid & 7];
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(scs + 4 * tid), "r"(w) : "memory");
+    }
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) mbar_init(&bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (tid == 0) {
+        asm volatile("st.shared.v2.u32 [%0], {%1,%2};" ::"r"(prod), "r"(b), "r"(nblk) : "memory");
+        asm volatile("st.shared.u32 [%0+8], %1;" ::"r"(prod), "r"(static_end) : "memory");
+        fence_proxy_async_global();  // (as staged_pass: the tables were written through the generic proxy)
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) produce(s);
+    }
+    const auto scalar = [&](int which) {
+        BindScalar r;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.w[i]) : "r"(scs + 32 * which + 4 * i));
+        return r;
+    };
+    const auto bind = [&](const Fr& lo, const Fr& hi, int which, bool h4) {
+        return h4 ? bind_pair<true>(lo, hi, scalar(which)) : bind_pair<false>(lo, hi, scalar(which));
+    };
+    uint64_t* const out = j ? tp.out[1] : tp.out[0];
+    const uint32_t ring = smem_u32(smem);
+    uint32_t A[17];
+#pragma unroll
+    for (int w = 0; w < 17; ++w) A[w] = 0;
+    for (uint32_t it = 0;; ++it) {
+        const int s = (int)(it % STG_STAGES);
+        mbar_wait(&bar[s], (it / STG_STAGES) & 1);
+        uint32_t t;
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(t) : "r"(smem_u32(tile_id + s)));
+        if (t == STG_NONE) break;
+        const uint32_t stage = ring + s * STG_STAGE_BYTES;
+        if (!BIND2) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                // this lane's quad of sub-step k; its entries (table jj, position ps) in the stage
+                uint32_t qa;
+                if (ORDER == ORDER_LOW_TO_HIGH) qa = stage + (lane & 3) * (SUB + 16) + ((lane >> 2) + 8 * k) * 4 * 32;
+                else qa = stage + (lane + 32 * k) * 32;
+                Fr x[2];
+#pragma unroll
+                for (int jj = 0; jj < 2; ++jj)
+                    x[jj] = look_operand(warp, [&](int ps) {
+                        const int u = ORDER == ORDER_LOW_TO_HIGH ? ps : ((ps & 1) << 1) | (ps >> 1);
+                        return lds_fr(qa + jj * TOFF + u * ESTEP);
+                    });
+                mul_wide_acc_reg(A, x[0].v, x[1].v);
+            }
+            __syncthreads();  // stage s is read out
+            if (tid == 0) produce(s);
+        } else {
+            Fr e[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) e[u] = lds_fr(stage + off + u * ESTEP);
+            __syncthreads();  // stage s is read out (and the exchange buffer of the previous tile)
+            if (tid == 0) produce(s);
+            Fr lo, hi;
+            if (ORDER == ORDER_LOW_TO_HIGH) {
+                lo = bind(e[0], e[1], 0, hi4a);
+                hi = bind(e[2], e[3], 0, hi4a);
+            } else {
+                lo = bind(e[0], e[2], 0, hi4a);
+                hi = bind(e[1], e[3], 0, hi4a);
+            }
+            const Fr v = bind(lo, hi, 1, hi4b);
+            const size_t y = ORDER == ORDER_LOW_TO_HIGH ? (size_t)t * STG_TILE + ty : (size_t)t * 32 + g + (size_t)(ty >> 5) * (n / 16);
+            stg_fr(out, y, v);
+#pragma unroll
+            for (int w = 0; w < 8; ++w)
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(xch + (((j * 4 + pos) * 8 + w) * 32 + g) * 4), "r"(v.v[w]) : "memory");
+            __syncthreads();
+            Fr x[2];
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj)
+                x[jj] = look_operand(warp, [&](int ps) {
+                    Fr r;
+#pragma unroll
+                    for (int w = 0; w < 8; ++w)
+                        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.v[w]) : "r"(xch + (((jj * 4 + ps) * 8 + w) * 32 + lane) * 4));
+                    return r;
+                });
+            mul_wide_acc_reg(A, x[0].v, x[1].v);
+        }
+    }
+    __syncthreads();  // every stage's last phase has been observed: no copy is in flight
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < STG_STAGES; ++s) mbar_inval(&bar[s]);
+    }
+    look_lanes_out(A, warp, lane, g_lanes, s_dst);
+}
+
+// Rounds whose tables hold `len` entries before their bind are folded into the next round's pass (their own
+// polynomial comes from the lookahead sums of the previous pass) when that pass is a staged one: a bind over
+// len / 2 entries that is not thin.
+__host__ __device__ inline bool res_fusable(uint64_t len) { return len / 4 > RES_THIN_PAIRS; }
+
 // lanes a member's round leaves in the accumulators / mailbox
 template <int D>
 __host__ __device__ constexpr int res_lanes(bool thin) {
@@ -543,6 +765,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
     constexpr int K = D;  // s(1) always comes from the running claim (the optimized tier's convention)
     extern __shared__ __align__(128) uint32_t dsm[];
     __shared__ uint64_t s_line[8];
+    __shared__ uint64_t s_chal2[4];
     __shared__ uint64_t* s_cur[RES_MAX_MEMBERS][T];
     __shared__ uint64_t* s_oth[RES_MAX_MEMBERS][T];
     __shared__ uint64_t s_len[RES_MAX_MEMBERS];
@@ -585,16 +808,28 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                 }
                 if (!got && lane == 1) v = RES_OP_ABORT;
                 if (lane < 8) s_line[lane] = v;
+                const bool two = got && (__shfl_sync(0xffffffffu, v, 1) & RES_FLAG_CHALLENGE2);
+                uint64_t c2 = 0;
+                if (two) {  // written before cmd_seq: behind a fence after the snapshot that showed cmd_seq
+                    __threadfence_system();
+                    if (lane < 4) c2 = reinterpret_cast<const volatile uint64_t*>(a.mb->challenge2[(seq + 1) & 1])[lane];
+                    if (lane < 4) s_chal2[lane] = c2;
+                }
                 if (live > 1) {  // re-publish for the other blocks: payload, then the sequence number (release)
-                    uint64_t w[7];
+                    uint64_t w[7], w2[4];
 #pragma unroll
                     for (int k = 0; k < 7; ++k) w[k] = __shfl_sync(0xffffffffu, v, k + 1);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) w2[k] = __shfl_sync(0xffffffffu, c2, k);
                     if (lane == 0) {
                         const long long t1 = clock64();
                         while (ld_acquire_gpu(&a.st->done) != seq)  // the previous round is complete
                             if (clock64() - t1 > a.timeout_cycles) break;
 #pragma unroll
                         for (int k = 0; k < 7; ++k) a.st->cmd[k] = w[k];
+                        if (two)
+#pragma unroll
+                            for (int k = 0; k < 4; ++k) a.st->challenge2[k] = w2[k];
                         st_release_gpu(&a.st->seq, seq + 1);
                     }
                 }
@@ -611,6 +846,9 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
             if (got) {
 #pragma unroll
                 for (int k = 0; k < 7; ++k) s_line[k + 1] = a.st->cmd[k];
+                if (s_line[1] & RES_FLAG_CHALLENGE2)
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) s_chal2[k] = a.st->challenge2[k];
             } else {
                 s_line[1] = RES_OP_ABORT;
             }
@@ -712,6 +950,38 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                     final_bind_pass<T, ORDER>(s_cur[m], s_oth[m], half, sc(), hi4, (uint64_t)b * sh.tpb + tid, (uint64_t)sh.nblk * sh.tpb);
                 continue;
             }
+            if constexpr (D == 2 && P == 1) if (act == RES_ACT_BIND2_EVAL || (act == RES_ACT_EVAL && (cmdw & RES_FLAG_LOOK))) {
+                const bool two = act == RES_ACT_BIND2_EVAL;
+                if (tid == 0) s_kl[m] = res_lanes<D>(true);
+                const ResShape sh = res_shape(len / 4, live);
+                if (b < sh.nblk) {
+                    TablePtrs tp;
+                    tp.in[0] = s_cur[m][0];
+                    tp.in[1] = s_cur[m][1];
+                    tp.out[0] = (ORDER == ORDER_LOW_TO_HIGH && two) ? s_oth[m][0] : s_cur[m][0];
+                    tp.out[1] = (ORDER == ORDER_LOW_TO_HIGH && two) ? s_oth[m][1] : s_cur[m][1];
+                    tp.e_out = tp.e_in = nullptr;
+                    tp.in_bits = 0;
+                    tp.work = a.st->work + m * 32;
+                    tp.static_end = ~(size_t)0;
+                    const uint32_t ntiles = (uint32_t)(len / 4 / STG_TILE);
+                    uint32_t static_end = ntiles;
+                    if (live > 1 && ntiles >= 2 * sh.nblk)
+                        static_end = (uint32_t)((uint64_t)ntiles * RES_STATIC_PCT / 100 / sh.nblk * sh.nblk);
+                    BindScalar s2;  // the member's pending challenge: bound first
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        s2.w[2 * i] = (uint32_t)s_chal2[i];
+                        s2.w[2 * i + 1] = (uint32_t)(s_chal2[i] >> 32);
+                    }
+                    const bool hi4_2 = (s_chal2[0] | s_chal2[1]) == 0;
+                    uint64_t* gl = a.st->lanes + m * RES_SLOT_U64;
+                    uint64_t* sl = live == 1 ? s_lanes + m * RES_SLOT_U64 : nullptr;
+                    const auto pass = two ? staged_look_pass<ORDER, true> : staged_look_pass<ORDER, false>;
+                    pass(tp, len, s2, sc(), hi4_2, hi4, reinterpret_cast<uint8_t*>(dsm), b, sh.nblk, static_end, gl, sl);
+                }
+                continue;
+            }
             const bool bind = act == RES_ACT_BIND_EVAL;
             const uint64_t nprime = bind ? len / 2 : len;
             const uint64_t pairs = nprime / 2;
@@ -781,7 +1051,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
             unsigned ln = 0;
             for (int m = 0; m < NM; ++m) {
                 const unsigned act = (eff_actions >> (4 * m)) & 0xf;
-                if (act == RES_ACT_BIND_EVAL || act == RES_ACT_FINAL) {
+                if (act == RES_ACT_BIND_EVAL || act == RES_ACT_FINAL || act == RES_ACT_BIND2_EVAL) {
                     if (ORDER == ORDER_LOW_TO_HIGH) {
 #pragma unroll
                         for (int j = 0; j < T; ++j) {
@@ -790,7 +1060,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                             s_oth[m][j] = t;
                         }
                     }
-                    s_len[m] /= 2;
+                    s_len[m] /= act == RES_ACT_BIND2_EVAL ? 4 : 2;
                 }
                 // largest pass this member can still ask for: an eval over len/2 pairs (not started) or a
                 // terminal bind over len/2 outputs
@@ -823,7 +1093,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                 for (int idx = tid; idx < NM * RES_SLOT_U64; idx += RES_BLOCK) {
                     const int m = idx / RES_SLOT_U64, i = idx % RES_SLOT_U64;
                     const unsigned act = (actions >> (4 * m)) & 0xf;
-                    if ((act == RES_ACT_EVAL || act == RES_ACT_BIND_EVAL) && i < s_kl[m]) {
+                    if ((act == RES_ACT_EVAL || act == RES_ACT_BIND_EVAL || act == RES_ACT_BIND2_EVAL) && i < s_kl[m]) {
                         s_lanes[idx] = __ldcg(a.st->lanes + idx);
                         a.st->lanes[idx] = 0;  // back to zero for the next round
                     }
@@ -871,7 +1141,7 @@ __global__ void __launch_bounds__(RES_BLOCK, 2) resident_rounds_kernel(const __g
                 for (int idx = pt; idx < NM * RES_SLOT_U64; idx += pn) {
                     const int m = idx / RES_SLOT_U64, i = idx % RES_SLOT_U64;
                     const unsigned act = (actions >> (4 * m)) & 0xf;
-                    if ((act == RES_ACT_EVAL || act == RES_ACT_BIND_EVAL) && i < s_kl[m]) result[idx] = s_lanes[idx];
+                    if ((act == RES_ACT_EVAL || act == RES_ACT_BIND_EVAL || act == RES_ACT_BIND2_EVAL) && i < s_kl[m]) result[idx] = s_lanes[idx];
                 }
             }
             // terminal binds that left a member fully bound hand the T values back with the acknowledgement
