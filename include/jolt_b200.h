@@ -508,6 +508,24 @@ typedef struct jb_lc_term {
 } jb_lc_term;
 int jb_table_linear_combination(jb_ctx* ctx, const jb_lc_term* terms, size_t count, size_t len, jb_table* out);
 
+/* Dory's vector-matrix product of a batched polynomial: the row combination v = L^T M of the joint polynomial
+ * P = sum_i c_i p_i (the terms, coefficients and prefix convention of jb_table_linear_combination) viewed as a matrix of
+ * R = len / W rows of W = row_width columns, flat index x = row W + col (the rows of jb_msm_g1_rows and
+ * jb_msm_g1_one_hot_rows):
+ *     v[col] = sum_{row < R} L[row] P[row W + col]
+ * P is never formed: each term is read once in its own format, and nothing of size len is allocated (len may exceed
+ * device memory: a one-hot term of K T = 2^32 entries costs its address column). A term shorter than W covers the
+ * first entries of row 0. left: a resident table of exactly R entries (any field values; Dory's is jb_eq_evals of the
+ * row coordinates), read and not modified. out: a NEW resident table of W entries, canonical, bit-exact and
+ * deterministic. Errors: every error of jb_table_linear_combination, checked the same way; JB_ERR_INVALID when
+ * row_width is not a power of two or exceeds len, and for an unknown left handle or one whose length is not
+ * len / row_width; JB_ERR_UNSUPPORTED unless count R < 2^32 (each column sums into 8 u64 lanes of 32-bit limb sums,
+ * which take at most 2^32 - 1 additions: one per row slice and up to R per cycle-major one-hot term). A one-hot
+ * address >= K that is not the none value is found on the device and returns JB_ERR_INVALID. After any error no table
+ * is created, nothing stays allocated and the context stays usable. */
+int jb_lc_vector_matrix_product(jb_ctx* ctx, const jb_lc_term* terms, size_t count, size_t len, size_t row_width,
+                                jb_table left, jb_table* out);
+
 /* Batch affine addition: batch_g1_additions_multi_affine (crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150),
  * the one-hot / binary column path of Dory's tier-1 commitments (crates/jolt-dory/src/streaming.rs:68,128,152,201).
  * Set s is indices[set_offsets[s] .. set_offsets[s + 1]) into `bases`; out_xy receives one AFFINE point per set

@@ -103,6 +103,8 @@ SIGNATURES = {
     "jb_one_hot_pushforward": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, c_size_t,
                                               c_size_t, ctypes.c_int, c_u64p, c_u64p]),
     "jb_table_linear_combination": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_u64p]),
+    "jb_lc_vector_matrix_product": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, ctypes.c_uint64,
+                                                   c_u64p]),
     "jb_ctx_diag": (ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_double)]),
     "jb_ctx_run_log": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.POINTER(c_size_t)]),
     "jb_ctx_timing_enable": (ctypes.c_int, [c_void_p, ctypes.c_int, ctypes.c_uint64]),

@@ -256,13 +256,26 @@ class Polynomial:
         if not terms:
             raise ValueError("linear_combination: at least one term")
         n = max(t.length for t in terms) if length is None else length
-        arr = (_lib.LcTermC * len(terms))()
-        keep = []
-        for i, t in enumerate(terms):
-            t._fill(arr[i], keep)
+        arr, keep = LinearTerm._array(terms)
         h = ctypes.c_uint64()
         session.check(session.lib.jb_table_linear_combination(session.h, ctypes.cast(arr, ctypes.c_void_p), len(terms),
                                                               n, ctypes.byref(h)))
+        return Polynomial(session, h.value)
+
+    @staticmethod
+    def vector_matrix_product(session: Session, terms: list["LinearTerm"], left: "Polynomial", row_width: int,
+                              length: int | None = None) -> "Polynomial":
+        """Dory's vector-matrix product v = L^T M of P = sum_i c_i p_i (the terms and prefix convention of
+        linear_combination, `length` defaulting to the longest term) laid out as length / row_width rows of row_width
+        columns: v[col] = sum_row left[row] P[row row_width + col], a new polynomial of row_width entries
+        (jb_lc_vector_matrix_product). P is never formed; `left` (length / row_width entries) is read, not modified."""
+        if not terms:
+            raise ValueError("vector_matrix_product: at least one term")
+        n = max(t.length for t in terms) if length is None else length
+        arr, keep = LinearTerm._array(terms)
+        h = ctypes.c_uint64()
+        session.check(session.lib.jb_lc_vector_matrix_product(session.h, ctypes.cast(arr, ctypes.c_void_p), len(terms),
+                                                              n, row_width, left.handle, ctypes.byref(h)))
         return Polynomial(session, h.value)
 
     @staticmethod
@@ -886,6 +899,15 @@ class LinearTerm:
             raise ValueError("LinearTerm.one_hot: one address column")
         return cls(_lib.JB_LC_ONE_HOT, K * T, coeff, ptr=ptrs[0], kind=kind, on_device=dev,
                    layout=ONE_HOT_LAYOUTS[layout], T=T, K=K, keep=keep)
+
+    @staticmethod
+    def _array(terms: list["LinearTerm"]):
+        """The jb_lc_term array of `terms`, and what must stay alive while the call reads it."""
+        arr = (_lib.LcTermC * len(terms))()
+        keep = []
+        for i, t in enumerate(terms):
+            t._fill(arr[i], keep)
+        return arr, keep
 
     def _fill(self, c, keep: list):
         c.type, c.kind, c.on_device, c.layout = self.type, self.kind, self.on_device, self.layout

@@ -29,6 +29,8 @@
 #include <vector>
 
 #include "columns.cuh"
+#include "lane_bins.cuh"
+#include "value_src.cuh"
 #include "member.hpp"
 
 using namespace jb;
@@ -48,37 +50,7 @@ struct EvalCol {  // one output of a launch: its source and its lane block
     uint64_t out;
 };
 
-// ---- value loaders: A += e * v(i) -----------------------------------------------------------------------------------
-struct FieldSrc {
-    static constexpr int SMEM_U4 = 1;
-    __device__ void init(uint4*) const {}
-    __device__ __forceinline__ void acc(uint32_t (&A)[17], const Fr& e, const void* p, size_t i, const uint4*) const {
-        const Fr v = ld_elem<Fr>(static_cast<const uint64_t*>(p), i);
-        mul_wide_acc_reg(A, e.v, v.v);
-    }
-};
-
-template <int KIND>
-struct SmallSrc {
-    static constexpr int SMEM_U4 = 1;
-    // 32-bit words of the magnitude
-    static constexpr int BW = KIND <= SK_U32 ? 1 : (KIND == SK_U64 || KIND == SK_I64 || KIND == SK_S64) ? 2 : 4;
-    __device__ void init(uint4*) const {}
-    __device__ __forceinline__ void acc(uint32_t (&A)[17], const Fr& e, const void* p, size_t i, const uint4*) const {
-        uint32_t mag[4];
-        const bool neg = ld_small(p, i, KIND, mag);
-        if (neg) {  // (p - e~) |v|: the Montgomery form of -e times |v|, still an exact non-negative integer product
-            uint32_t ne[8];
-            const uint32_t pm[8] = {FrParams::P(0), FrParams::P(1), FrParams::P(2), FrParams::P(3),
-                                    FrParams::P(4), FrParams::P(5), FrParams::P(6), FrParams::P(7)};
-            sub8(ne, pm, e.v);
-            mul_wide_acc_bw<BW>(A, ne, mag);
-        } else {
-            mul_wide_acc_bw<BW>(A, e.v, mag);
-        }
-    }
-};
-
+// ---- value loaders: A += e * v(i) (field and compact values: value_src.cuh) ------------------------------------
 // v_j = eq(r_addr, addr_j), 0 for the none value; an address >= K that is not none raises *bad and counts as 0.
 template <int KIND, bool SMEM>
 struct OneHotSrc {
@@ -146,20 +118,6 @@ __global__ void __launch_bounds__(EV_BLOCK, 2)
     }
 }
 
-// Warp-aggregated bin update: every thread with emit adds its field value `v` (8 canonical limbs) to bin `key`.
-__device__ __forceinline__ void pf_flush(bool emit, uint32_t key, const Fr& v, unsigned long long* bins, int lane) {
-    const unsigned m = __ballot_sync(0xffffffffu, emit);
-    if (!emit) return;
-    const unsigned peers = __match_any_sync(m, key);
-    const int leader = __ffs(peers) - 1;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-        const uint32_t lo = __reduce_add_sync(peers, v.v[w] & 0xffffu);
-        const uint32_t hi = __reduce_add_sync(peers, v.v[w] >> 16);
-        if (lane == leader) atomicAdd(bins + (size_t)key * 8 + w, (unsigned long long)lo + ((unsigned long long)hi << 16));
-    }
-}
-
 // lanes: count x K x 8 (zeroed); the grid is that of mle_eval_kernel over the T cycles.
 template <int KIND, bool SMEM>
 __global__ void __launch_bounds__(EV_BLOCK)
@@ -206,27 +164,6 @@ __global__ void __launch_bounds__(EV_BLOCK)
                 if (s_bins[i]) atomicAdd(g_bins + i, s_bins[i]);
             __syncthreads();
         }
-    }
-}
-
-// n bins of 8 u64 limb-sum lanes -> canonical Montgomery elements (the lanes hold sums of Montgomery values, so the
-// integer they encode is reduced mod p, not Montgomery-reduced): V = lo + top 2^256, V mod p = (lo mod p) + top R.
-__global__ void __launch_bounds__(EV_BLOCK) bins_to_fr_kernel(const unsigned long long* lanes, size_t n, uint64_t* out) {
-    for (size_t i = (size_t)blockIdx.x * EV_BLOCK + threadIdx.x; i < n; i += (size_t)gridDim.x * EV_BLOCK) {
-        Fr lo, top = Fr::zero();
-        unsigned long long carry = 0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) {
-            const unsigned long long v = lanes[i * 8 + w];
-            const unsigned long long s = (v & 0xffffffffull) + (carry & 0xffffffffull);
-            lo.v[w] = (uint32_t)s;
-            carry = (v >> 32) + (carry >> 32) + (s >> 32);
-        }
-        top.v[0] = (uint32_t)carry;
-        top.v[1] = (uint32_t)(carry >> 32);
-#pragma unroll
-        for (int k = 0; k < 5; ++k) cond_sub_p<FrParams>(lo.v);  // lo < 2^256 < 6p
-        st_elem(out, i, fp_add(lo, fp_mul(top, Fr::r2())));  // top < 2^64 < p: montmul(top, R^2) = top R mod p
     }
 }
 
@@ -472,7 +409,7 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
         const jb_table h = c->next_id++;
         c->tables[h] = t;
         made.push_back(h);
-        bins_to_fr_kernel<<<launch_grid(c, K, EV_BLOCK, 8), EV_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, t.buf);
+        bins_to_fr_kernel<<<launch_grid(c, K, BINS_BLOCK, 8), BINS_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, t.buf);
         c->launches++;
         st = c->check(cudaGetLastError(), "bins_to_fr_kernel launch");
     }
