@@ -126,6 +126,19 @@ int jb_eq_evals(jb_ctx* ctx, const uint64_t* r, size_t nvars, const uint64_t* sc
 /* EqPolynomial::evals_for_aligned_block (eq.rs:238-263): the per-GPU slice of a sharded eq table. */
 int jb_eq_evals_aligned_block(jb_ctx* ctx, const uint64_t* r, size_t nvars, size_t start_index,
                               size_t block_size, jb_table* out);
+/* The structured factors of the value-evaluation and shift relations, as new tables of 2^nvars entries. Both are
+ * linear maps of E[t] = scale * eq(r, t) with jb_eq_evals' conventions (r[0] <-> most-significant index bit,
+ * canonical Montgomery limbs, [0,0,lo,hi] challenges take the half-cost path, scale_or_null == NULL means 1):
+ *   jb_lt_evals:          LT[j] = sum_{t > j} E[t]  = scale * LT(j, r),       LT(x, y) = sum_i (1 - x_i) y_i prod_{k<i} eq(x_k, y_k)
+ *   jb_eq_plus_one_evals: E1[j] = E[j - 1], E1[0] = 0 = scale * EqPlusOne(r, j),
+ *                         EqPlusOne(x, y) = sum_i prod_{k<i} eq(x_k, y_k) (1 - x_i) y_i prod_{k>i} x_k (1 - y_k)
+ *                         (1 iff y = x + 1 on the cube).
+ * Value evaluation: Val(r_addr, r_cycle) = sum_j inc(j) wa(r_addr, j) LT(j, r_cycle) takes jb_lt_evals(r_cycle).
+ * Shift: NextPC(r) = sum_j EqPlusOne(r, j) PC(j) takes jb_eq_plus_one_evals(r). For nvars = 0 both are [0].
+ * Errors as jb_eq_evals: JB_ERR_INVALID (null pointer, non-canonical limbs, nvars > 40), JB_ERR_OOM, JB_ERR_NO_DEVICE
+ * (no context without a device); after an error no table exists and the context stays usable. */
+int jb_lt_evals(jb_ctx* ctx, const uint64_t* r, size_t nvars, const uint64_t* scale_or_null, jb_table* out);
+int jb_eq_plus_one_evals(jb_ctx* ctx, const uint64_t* r, size_t nvars, const uint64_t* scale_or_null, jb_table* out);
 
 /* ---- sumcheck member: ProveRounds (crates/jolt-sumcheck/src/prover.rs:52-72) for the
  *      product-of-m-tables relation, degree m (naive.rs:241-316; tests/roundtrip.rs:26-97) ------- */

@@ -17,6 +17,7 @@ from .api import (  # noqa: F401
     SCALAR_KINDS,
     Source,
     BatchMember,
+    EqPlusOnePolynomial,
     EqPolynomial,
     EqProductMember,
     ExpressionMember,
@@ -24,6 +25,7 @@ from .api import (  # noqa: F401
     HyperKZG,
     HyperKZGProof,
     LinearTerm,
+    LtPolynomial,
     Polynomial,
     ProductMember,
     ProductSourcesMember,

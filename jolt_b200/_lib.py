@@ -40,6 +40,8 @@ SIGNATURES = {
                                            ctypes.POINTER(ctypes.c_uint64)]),
     "jb_eq_evals": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_u64p, c_u64p]),
     "jb_eq_evals_aligned_block": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_size_t, c_size_t, c_u64p]),
+    "jb_lt_evals": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_u64p, c_u64p]),
+    "jb_eq_plus_one_evals": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_u64p, c_u64p]),
     "jb_member_create": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_create_sop": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, c_size_t, ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_num_tables": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_size_t)]),

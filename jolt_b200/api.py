@@ -444,6 +444,66 @@ class EqPolynomial:
         return Polynomial(session, h.value)
 
 
+def _structured_evals(session: Session, fn, r_limbs, scaling_factor) -> Polynomial:
+    r = np.ascontiguousarray(r_limbs, dtype=np.uint64).reshape(-1, 4)
+    sc = None if scaling_factor is None else _limbs(scaling_factor)
+    h = ctypes.c_uint64()
+    session.check(fn(session.h, _p(r) if r.shape[0] else None, r.shape[0], _p(sc) if sc is not None else None,
+                     ctypes.byref(h)))
+    return Polynomial(session, h.value)
+
+
+def _coords(x, y) -> tuple[list[int], list[int]]:
+    x, y = [int(v) % F.R_MOD for v in x], [int(v) % F.R_MOD for v in y]
+    if len(x) != len(y):
+        raise ValueError("the two points must have the same number of coordinates")
+    return x, y
+
+
+class LtPolynomial:
+    """LT(x, y) = sum_i (1 - x_i) y_i prod_{k<i} eq(x_k, y_k), x[0] / y[0] <-> MSB: on the cube, 1 iff x < y.
+    evals(r) is the table LT(j, r) (= sum_{t > j} eq(r, t)), the factor of value evaluation
+    Val(r_addr, r_cycle) = sum_j inc(j) wa(r_addr, j) LT(j, r_cycle); after a sumcheck binds it at rho, its final
+    value is scale * evaluate(rho, r)."""
+
+    @staticmethod
+    def evals(session: Session, r_limbs, scaling_factor=None) -> Polynomial:
+        return _structured_evals(session, session.lib.jb_lt_evals, r_limbs, scaling_factor)
+
+    @staticmethod
+    def evaluate(x, y) -> int:
+        x, y = _coords(x, y)
+        p, acc, pre = F.R_MOD, 0, 1
+        for a, b in zip(x, y):
+            acc = (acc + (1 - a) * b * pre) % p
+            pre = pre * (a * b + (1 - a) * (1 - b)) % p
+        return acc
+
+
+class EqPlusOnePolynomial:
+    """EqPlusOne(x, y) = sum_i prod_{k<i} eq(x_k, y_k) (1 - x_i) y_i prod_{k>i} x_k (1 - y_k), x[0] / y[0] <-> MSB:
+    on the cube, 1 iff y = x + 1. evals(r) is the table EqPlusOne(r, j) (= eq(r, j - 1), 0 at j = 0), the factor of a
+    shift NextPC(r) = sum_j EqPlusOne(r, j) PC(j); after a sumcheck binds it at rho, its final value is
+    scale * evaluate(r, rho)."""
+
+    @staticmethod
+    def evals(session: Session, r_limbs, scaling_factor=None) -> Polynomial:
+        return _structured_evals(session, session.lib.jb_eq_plus_one_evals, r_limbs, scaling_factor)
+
+    @staticmethod
+    def evaluate(x, y) -> int:
+        x, y = _coords(x, y)
+        p, n = F.R_MOD, len(x)
+        suf = [1] * (n + 1)  # suf[i] = prod_{k >= i} x_k (1 - y_k)
+        for i in range(n - 1, -1, -1):
+            suf[i] = suf[i + 1] * x[i] * (1 - y[i]) % p
+        acc, pre = 0, 1
+        for i in range(n):
+            acc = (acc + pre * (1 - x[i]) * y[i] * suf[i + 1]) % p
+            pre = pre * (x[i] * y[i] + (1 - x[i]) * (1 - y[i])) % p
+        return acc
+
+
 class UnivariatePoly:
     """jolt_poly::UnivariatePoly (univariate.rs:27): coefficients ascending, values as ints mod r.
     Stays on the host in the reference too (O(d^2) work on <= ~10 elements)."""

@@ -68,28 +68,7 @@ int jbi::bind_table(jb_ctx* c, Table& t, const uint64_t r[4], int order) {
 }
 
 
-namespace {
 // eq table for `nvars` variables (HOST limbs r, optional host scale); recursive prefix for n > 11.
-EqVars eq_vars(const uint64_t* r, size_t count, const uint64_t* scale) {
-    EqVars v;
-    std::memset(&v, 0, sizeof v);
-    for (size_t j = 0; j < count; ++j)
-        for (int w = 0; w < 4; ++w) {
-            v.r[j][2 * w] = (uint32_t)r[4 * j + w];
-            v.r[j][2 * w + 1] = (uint32_t)(r[4 * j + w] >> 32);
-        }
-    if (scale) {
-        v.has_scale = 1;
-        for (int w = 0; w < 4; ++w) {
-            v.scale[2 * w] = (uint32_t)scale[w];
-            v.scale[2 * w + 1] = (uint32_t)(scale[w] >> 32);
-        }
-    }
-    return v;
-}
-
-}  // namespace
-
 int jbi::eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, uint64_t* d_out) {
     if (nvars <= (size_t)EQ_BLOCK_VARS) {
         eq_expand_kernel<<<1, 256, 0, c->stream>>>(nullptr, eq_vars(r, nvars, scale), (int)nvars, d_out);

@@ -33,6 +33,25 @@ inline BindScalar make_scalar(const uint64_t r[4], bool* hi4) {
 
 inline bool canonical_fr(const uint64_t r[4]) { return !HostFr::geq_p(r); }
 
+// The kernel-parameter form of `count` <= EQ_BLOCK_VARS coordinates (HOST limbs r) and an optional host scale.
+inline jb::EqVars eq_vars(const uint64_t* r, size_t count, const uint64_t* scale) {
+    jb::EqVars v;
+    std::memset(&v, 0, sizeof v);
+    for (size_t j = 0; j < count; ++j)
+        for (int w = 0; w < 4; ++w) {
+            v.r[j][2 * w] = (uint32_t)r[4 * j + w];
+            v.r[j][2 * w + 1] = (uint32_t)(r[4 * j + w] >> 32);
+        }
+    if (scale) {
+        v.has_scale = 1;
+        for (int w = 0; w < 4; ++w) {
+            v.scale[2 * w] = (uint32_t)scale[w];
+            v.scale[2 * w + 1] = (uint32_t)(scale[w] >> 32);
+        }
+    }
+    return v;
+}
+
 // Launches one round of a per-round sumcheck kernel over `pairs` pair indices: `kernel(args..., out)`, whose blocks
 // each leave `values` partial sums in the context's partial buffer for the last block to fold. `kind` and `m` label
 // the timed launch (jb_ctx::timing_begin), `what` names a launch error.
