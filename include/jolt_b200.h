@@ -275,6 +275,49 @@ int jb_member_create_expr_sources(jb_ctx* ctx, const jb_source* sources, size_t 
 int jb_member_create_product_sources(jb_ctx* ctx, const jb_source* sources, size_t nsources, size_t len,
                                      const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null,
                                      int order, jb_member** out);
+/* Read-write checking member (Twist read / write checking of RAM or registers): ProveRounds for
+ *   sum_{k<K} sum_{j<T} scale * eq(w_cycle, j) * sum_a c_a * ra_a(k, j) * (Val(k, j) + d_a * inc(j)),
+ * over the sparse K x T memory matrix, index x = k * T + j, holding O(A * T) memory and never K * T. With
+ *   ra_a(k, j) = [addr_a(j) = k],   Val(k, j) = init(k) + sum_{j' < j, addr_w(j') = k} inc(j'),
+ * access a = 0 .. A-1 (1 <= A <= JB_RW_MAX_ACCESSES) reads its address column addr_a, its value column v_a, its
+ * coefficient c_a and its flag d_a in {0, 1}; access w is the write. Two accesses may share an address column: RAM is
+ * one column used twice, (c = 1, d = 0) for the read and (c = gamma, d = 1) for the write; registers are rs1, rs2, rd.
+ *  - T = 2^t cycles, 2 <= T <= 2^30; K = 2^kappa addresses, 1 <= K <= 2^16; min(K, distinct address columns) * T <
+ *    2^31. Address columns: T entries of addr_kind (JB_SCALAR_U8 / U16; the all-ones value means no access), all in
+ *    host memory or all in device memory (addr_on_device), aligned to their entry.
+ *  - Values (T entries), inc (T entries) and init (K entries) are jb_sources of type JB_SOURCE_TABLE (a field table,
+ *    left to the caller) or JB_SOURCE_COMPACT (a compact column of any jb_scalar_kind but JB_SCALAR_FR, e.g. inc as
+ *    i64 / i128 / S64 / S128). Every column and table is borrowed for the call only.
+ *  - Precondition, relied on and not checked (checking needs a sort by address; a prover trusts its witness the same
+ *    way): v_a(j) = Val(addr_a(j), j) wherever addr_a(j) is not none - the read values the witness holds.
+ *  - w_cycle: nvars = t coordinates, w[0] <-> the most significant bit of j; optional scale. Variables are bound
+ *    LowToHigh on x (the only order): first the t cycle bits, LSB first, then the kappa address bits.
+ *  - degree 3; t + kappa rounds; the running claim is mandatory in prove_round. The cycle rounds keep the eq factor
+ *    split as jb_eq_member_create does and cost O(live entries) each: the matrix is kept as entries per (row, address)
+ *    and a round pairs adjacent rows. After the t-th bind the one remaining row becomes K-entry field tables and the
+ *    address rounds run as an expression member (their polynomial has degree 2; the degree-3 evaluations are
+ *    published).
+ *  - jb_member_final_evals returns A + 2 values: ra_0 .. ra_{A-1} at (r_addr, r_cycle), then Val(r_addr, r_cycle),
+ *    then inc(r_cycle) - the claims of the value-evaluation, RA and increment-reduction sumchecks.
+ *    jb_eq_member_scalar returns scale * eq(w_cycle, r_cycle) once the cycle rounds are done.
+ *  - Everything the rounds need is allocated at creation, so JB_ERR_OOM can only arise here.
+ * Errors, with nothing left allocated: JB_ERR_UNSUPPORTED for HighToLow and A > JB_RW_MAX_ACCESSES; JB_ERR_INVALID for
+ * A = 0, write_access >= A, an unknown order, an unknown or misaligned column kind, on_device not 0 / 1, T or K not a
+ * power of two or out of range, a table of another length, nvars != t, a non-canonical coefficient, point or scale, a
+ * write_flag not 0 / 1, a null pointer; and, found on the device at creation, an address >= K that is not none or a
+ * nonzero inc(j) at a cycle whose write address is none. The member works in jb_prove_batch and jb_scheduler_*; it never
+ * runs in a resident kernel and is not sharded (jb_member_prove_round_partials returns JB_ERR_UNSUPPORTED). */
+#define JB_RW_MAX_ACCESSES 4
+typedef struct jb_rw_access {
+    const void* addr;         /* T addresses of the call's addr_kind */
+    jb_source value;          /* v_a: JB_SOURCE_TABLE or JB_SOURCE_COMPACT, T entries */
+    uint64_t coeff[4];        /* c_a, Montgomery limbs, canonical */
+    int write_flag;           /* d_a: 1 adds inc(j) to the value this access sees */
+} jb_rw_access;
+int jb_member_create_read_write(jb_ctx* ctx, const jb_rw_access* accesses, size_t naccesses, size_t write_access,
+                                int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
+                                const jb_source* init, const uint64_t* w_cycle, size_t nvars, const uint64_t* scale_or_null,
+                                int order, jb_member** out);
 /* Multi-GPU: like prove_round but leaves this rank's partial sums - the kernel values s(0), [s(1) unless
  * skip_t1], s(2), .., s(m-1), s(inf) in the order jb_round_evals_from_kernel_values documents - on the device as
  * count x 8 uint64 lanes, each holding one 32-bit limb (exact under ncclSum over <= 2^32 ranks); the caller

@@ -30,6 +30,7 @@ from .api import (  # noqa: F401
     ProductMember,
     ProductSourcesMember,
     ProvedBatch,
+    ReadWriteCheckingMember,
     RoundScheduler,
     Session,
     SumOfProductsMember,

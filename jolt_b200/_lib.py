@@ -64,6 +64,9 @@ SIGNATURES = {
                                                      c_size_t, c_u64p, ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_create_product_sources": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_u64p, c_size_t, c_u64p,
                                                         ctypes.c_int, ctypes.POINTER(c_void_p)]),
+    "jb_member_create_read_write": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, ctypes.c_int, ctypes.c_int,
+                                                   c_size_t, c_size_t, c_void_p, c_void_p, c_u64p, c_size_t, c_u64p,
+                                                   ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_member_prove_round_partials": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, c_void_p]),
     "jb_ctx_set_verify_rounds": (ctypes.c_int, [c_void_p, ctypes.c_int]),
     "jb_partials_finalize": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_u64p]),
@@ -157,6 +160,13 @@ JB_SOURCE_TABLE, JB_SOURCE_COMPACT, JB_SOURCE_ONE_HOT = 0, 1, 2
 class SourceC(ctypes.Structure):
     _fields_ = [("type", ctypes.c_int), ("kind", ctypes.c_int), ("on_device", ctypes.c_int), ("table", ctypes.c_uint64),
                 ("values", c_void_p), ("K", c_size_t), ("r_addr", c_u64p)]
+
+
+JB_RW_MAX_ACCESSES = 4
+
+
+class RwAccessC(ctypes.Structure):
+    _fields_ = [("addr", c_void_p), ("value", SourceC), ("coeff", ctypes.c_uint64 * 4), ("write_flag", ctypes.c_int)]
 
 
 JB_LC_TABLE, JB_LC_COMPACT, JB_LC_ONE_HOT = 0, 1, 2

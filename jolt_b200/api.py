@@ -867,6 +867,45 @@ class ProductSourcesMember(ExpressionMember):
         return self
 
 
+class ReadWriteCheckingMember(ExpressionMember):
+    """Twist read-write checking (jb_member_create_read_write): ProveRounds for
+      sum_{k<K} sum_{j<T} scale * eq(w_cycle, j) * sum_a c_a * ra_a(k, j) * (Val(k, j) + d_a * inc(j))
+    over the sparse K x T memory matrix, from the witness columns, in O(A T) memory. ra_a(k, j) = [addr_a(j) = k];
+    Val(k, j) = init(k) + the increments of the earlier cycles whose write address is k. `accesses`: up to 4 tuples
+    (addresses, values, coeff, d) - a uint8 / uint16 address column (the all-ones value = no access; accesses may share
+    one column), the values v_a(j) = Val(addr_a(j), j) the witness holds (a Source.table or Source.compact, or anything
+    Source.compact takes), c_a (an int or 4 Montgomery limbs) and d_a in {0, 1}; access `write` is the write. `inc`
+    (T entries) and `init` (K entries) likewise. Everything is borrowed for the call. Degree 3, log2 T + log2 K rounds,
+    LowToHigh only; the running claim is mandatory. final_evals() returns ra_0 .. ra_{A-1}, Val, inc at the point."""
+
+    def __init__(self, session: Session, accesses, write: int, inc, init, K: int, w_cycle, scale=None,
+                 order: int = LOW_TO_HIGH):
+        def src(x):
+            return x if isinstance(x, Source) else Source.compact(x)
+        ptrs, kind, T, dev, keep = _address_columns([a[0] for a in accesses], "ReadWriteCheckingMember")
+        arr = (_lib.RwAccessC * max(len(accesses), 1))()
+        for i, (_addr, values, coeff, d) in enumerate(accesses):
+            arr[i].addr = ptrs[i]
+            src(values)._fill(arr[i].value, keep)
+            arr[i].coeff[:] = [int(x) for x in _limbs(coeff % F.R_MOD if isinstance(coeff, (int, np.integer)) else coeff)]
+            arr[i].write_flag = int(d)
+        inc_c, init_c = _lib.SourceC(), _lib.SourceC()
+        src(inc)._fill(inc_c, keep)
+        src(init)._fill(init_c, keep)
+        w = point_limbs(w_cycle)
+        sc = None if scale is None else _limbs(scale)
+        h = ctypes.c_void_p()
+        session.check(session.lib.jb_member_create_read_write(
+            session.h, ctypes.cast(arr, ctypes.c_void_p), len(accesses), write, kind, dev, T, K,
+            ctypes.cast(ctypes.pointer(inc_c), ctypes.c_void_p), ctypes.cast(ctypes.pointer(init_c), ctypes.c_void_p),
+            _p(w) if w.shape[0] else None, w.shape[0], _p(sc) if sc is not None else None, order, ctypes.byref(h)))
+        self.s = session
+        self.h = h
+        self.ntables = len(accesses) + 2
+        self._degree = 3
+        self.m = 3
+
+
 def _monomials_c(monomials):
     mons = (_lib.MonomialC * max(len(monomials), 1))()
     for k, (coeff, tabs) in enumerate(monomials):

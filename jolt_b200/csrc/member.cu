@@ -229,6 +229,39 @@ static void* const JB_LANES_EXCHANGE = (void*)(uintptr_t)1;  // sentinel: all-re
 
 using EqRound = EqWeights;
 
+// Where a launched round pass reports: result slot `slot`, device lanes (lanes_out) or the peer exchange.
+static RoundOut round_out(jb_ctx* c, void* lanes_out, int slot, uint64_t* seq_out) {
+    RoundOut ro;
+    ro.partial = nullptr;  // set by launch_round
+    ro.counter = c->d_counter;
+    ro.lanes = lanes_out ? 1 : 0;
+    ro.world = 1;
+    ro.rank = 0;
+    ro.xseq = 0;
+    ro.timeout_cycles = 0;
+    for (int g2 = 0; g2 < 16; ++g2) ro.peer[g2] = nullptr;
+    ro.seq = ++c->result_seq;
+    if (seq_out) *seq_out = ro.seq;
+    uint64_t* slot_dev = c->d_result_alias + (size_t)slot * JB_SLOT_U64;
+    if (lanes_out == JB_LANES_EXCHANGE) {  // fused all-reduce over peer memory, totals (lanes) to the host
+        ro.lanes = 2;
+        ro.result = slot_dev;
+        ro.flag = slot_dev + 64;
+        for (int g2 = 0; g2 < 16; ++g2) ro.peer[g2] = c->xch_peer[g2];
+        ro.world = c->world;
+        ro.rank = c->rank;
+        ro.xseq = ++c->xch_seq;
+        ro.timeout_cycles = 20000000000LL;
+    } else if (lanes_out) {
+        ro.result = (uint64_t*)lanes_out;
+        ro.flag = nullptr;
+    } else {
+        ro.result = slot_dev;
+        ro.flag = slot_dev + 64;
+    }
+    return ro;
+}
+
 static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* lanes_out, const EqRound* eqr = nullptr,
                         int slot = 0, uint64_t* seq_out = nullptr) {
     jb_ctx* c = mem->ctx;
@@ -272,34 +305,7 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
             tp.in[j] = ins[j];
             tp.out[j] = outs[j];
         }
-    RoundOut ro;
-    ro.partial = nullptr;  // set by launch_round
-    ro.counter = c->d_counter;
-    ro.lanes = lanes_out ? 1 : 0;
-    ro.world = 1;
-    ro.rank = 0;
-    ro.xseq = 0;
-    ro.timeout_cycles = 0;
-    for (int g2 = 0; g2 < 16; ++g2) ro.peer[g2] = nullptr;
-    ro.seq = ++c->result_seq;
-    if (seq_out) *seq_out = ro.seq;
-    uint64_t* slot_dev = c->d_result_alias + (size_t)slot * JB_SLOT_U64;
-    if (lanes_out == JB_LANES_EXCHANGE) {  // fused all-reduce over peer memory, totals (lanes) to the host
-        ro.lanes = 2;
-        ro.result = slot_dev;
-        ro.flag = slot_dev + 64;
-        for (int g2 = 0; g2 < 16; ++g2) ro.peer[g2] = c->xch_peer[g2];
-        ro.world = c->world;
-        ro.rank = c->rank;
-        ro.xseq = ++c->xch_seq;
-        ro.timeout_cycles = 20000000000LL;
-    } else if (lanes_out) {
-        ro.result = (uint64_t*)lanes_out;
-        ro.flag = nullptr;
-    } else {
-        ro.result = slot_dev;
-        ro.flag = slot_dev + 64;
-    }
+    const RoundOut ro = round_out(c, lanes_out, slot, seq_out);
     int st;
     if (mem->product) {
         st = product_round(c, mem, ins, outs, eqr, eqr ? true : skip1, pairs, do_bind, hi4, s, ro);
@@ -673,10 +679,13 @@ static void eq_absorb_bind(jb_member* mem, size_t var, const uint64_t* r) {
     (HostFr::from_limbs(mem->eq_scalar) * f).store(mem->eq_scalar);
 }
 
+static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
+
 static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
     jb_ctx* c = mem->ctx;
     if (!claim) return c->fail(JB_ERR_INVALID, "eq member: the running claim is required (Gruen hint s(0)+s(1))");
     const size_t n = mem->eq_n, M = (size_t)mem->m;
+    if (mem->rw && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
     if (round >= n) return c->fail(JB_ERR_INVALID, "prove_round: member is fully bound");
     const bool l2h = mem->order == JB_LOW_TO_HIGH;
     if (bind) {
@@ -712,7 +721,8 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     const HostFr wc = HostFr::from_limbs(mem->eq_w.data() + 4 * cur_var);
     const HostFr l1 = scalar * wc, l0 = scalar - l1;
     if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
-    int st = member_round(mem, bind, true, nullptr, &er);
+    int st = mem->rw ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+                     : member_round(mem, bind, true, nullptr, &er);
     if (st != JB_OK) return st;
     // a field inversion is ~400 host multiplications (~13 us): do it while the device runs the pass (the
     // extrapolation constants below are built once)
@@ -1071,6 +1081,71 @@ int jb_member_create_product_sources(jb_ctx* c, const jb_source* sources, size_t
     return create_over_sources(c, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null, order, check, shape, out);
 }
 
+// ---- read-write checking member -------------------------------------------------------------------------
+// Binds a cycle variable of a read-write member (its eq factor has absorbed r); after the last one the member becomes
+// an expression member over its K-entry tables ra_0 .. ra_{A-1}, Val, inc: sum_k e sum_a c_a ra_a(k) (Val(k) + d_a inc)
+// with e = scale * eq(w_cycle, r_cycle), as monomials c_a e ra_a Val and c_a e ra_a inc.
+static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
+    const RwState& rw = *mem->rw;
+    const int A = rw.A;
+    int st = rw_cycle_bind(mem, r);
+    if (st != JB_OK || rw.rows > 1) return st;
+    const HostFr e = HostFr::from_limbs(mem->eq_scalar);
+    jb_monomial mo[2 * RW_MAX_ACCESSES];
+    size_t nm = 0;
+    for (int a = 0; a < A; ++a)
+        for (int k = 0; k < 1 + rw.d[a]; ++k) {
+            std::memset(&mo[nm], 0, sizeof mo[nm]);
+            (HostFr::from_limbs(rw.coeff[a]) * e).store(mo[nm].coeff);
+            mo[nm].degree = 2;
+            mo[nm].table[0] = (uint32_t)a;
+            mo[nm].table[1] = (uint32_t)(A + k);
+            ++nm;
+        }
+    make_expr(mem, mo, nm, (size_t)A + 2, 2);
+    return JB_OK;
+}
+
+// An address round: the first one binds the last cycle variable and hands the member over to its expression pass.
+// The round polynomial has degree 2; s(3) is extrapolated so the member keeps reporting degree 3.
+static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
+    jb_ctx* c = mem->ctx;
+    if (round == mem->eq_n) {
+        eq_absorb_bind(mem, 0, bind);
+        const int st = rw_bind_cycle(mem, bind);
+        if (st != JB_OK) return st;
+        bind = nullptr;
+    }
+    const bool skip1 = !c->verify_rounds;
+    int st = member_round(mem, bind, skip1, nullptr);
+    if (st == JB_OK) st = wait_round_result0(c);
+    if (st != JB_OK) return st;
+    uint64_t vals[JB_MAX_ROUND_EVALS * 4];
+    st = assemble_evals(c, 2, skip1, slot_values(c->h_result, 2, skip1, vals), claim, round, out_evals);  // s(0..2)
+    if (st != JB_OK) return st;
+    const RoundConsts& rc = round_consts(2);
+    HostFr s3 = HostFr::zero();
+    for (int t = 0; t <= 2; ++t) s3 = s3 + rc.next[t] * HostFr::from_limbs(out_evals + 4 * t);
+    s3.store(out_evals + 12);
+    return JB_OK;
+}
+
+int jb_member_create_read_write(jb_ctx* c, const jb_rw_access* accesses, size_t naccesses, size_t write_access,
+                                int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
+                                const jb_source* init, const uint64_t* w_cycle, size_t nvars, const uint64_t* scale_or_null,
+                                int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    jb_member* mem = nullptr;
+    {
+        Guard g(c);
+        const int st = rw_create(c, accesses, naccesses, write_access, addr_kind, addr_on_device, T, K, inc, init, w_cycle,
+                                 nvars, scale_or_null, order, &mem);
+        if (st != JB_OK) return st;
+    }
+    *out = mem;
+    return eq_setup(mem, w_cycle, nvars, scale_or_null, out);
+}
+
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
 int jb_eq_member_scalar(jb_member* mem, uint64_t out[4]) {
     if (!mem || !out || !mem->eq) return JB_ERR_INVALID;
@@ -1240,6 +1315,7 @@ int jb_member_prove_round_partials(jb_member* mem, const uint64_t* bind, size_t 
     Guard g(mem->ctx, true);
     if (mem->expr) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: expression members are not sharded");
     if (mem->product) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: product members are not sharded");
+    if (mem->rw) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: read-write members are not sharded");
     before_launch(mem);
     return member_round(mem, bind, skip_t1 != 0, lanes_out);
 }
@@ -1349,6 +1425,7 @@ int jb_member_export_table(jb_member* mem, size_t j, void* device_dst, size_t ca
     Guard g(c, true);
     before_launch(mem);  // the host's view of the tables (buffer parity, length) is exact at a round boundary
     if (j >= (size_t)mem->ntables()) return c->fail(JB_ERR_INVALID, "export_table: table index out of range");
+    if (mem->rw && !mem->expr) return c->fail(JB_ERR_INVALID, "export_table: a read-write member in its cycle rounds has no tables");
     if (!mem->src.empty() && mem->src[j].type != JB_SOURCE_TABLE)
         return c->fail(JB_ERR_INVALID, "export_table: the source is not bound yet (a column, not a field table)");
     if (cap_elems < mem->len) return c->fail(JB_ERR_INVALID, "export_table: destination too small");
@@ -1367,7 +1444,12 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     Guard g(c, true);
     if (mem->len < 2) return c->fail(JB_ERR_INVALID, "finish_rounds: member already fully bound");
     if (!canonical_fr(bind)) return c->fail(JB_ERR_INVALID, "finish_rounds: challenge limbs not canonical");
-    if (mem->eq) {
+    if (mem->rw && !mem->expr) {  // K = 1: the last cycle variable is the member's last
+        if (mem->len != 2) return c->fail(JB_ERR_INVALID, "finish_rounds: rounds remain");
+        eq_absorb_bind(mem, 0, bind);
+        return rw_bind_cycle(mem, bind);
+    }
+    if (mem->eq && !mem->rw) {
         size_t var = 0;
         for (size_t l = mem->len; l > 2; l >>= 1) ++var;  // unbound variables besides the one being bound
         // LowToHigh binds w[var] (the most significant unbound one is w[0]); HighToLow binds w[n - 1 - var]
@@ -1433,6 +1515,8 @@ void jb_member_destroy(jb_member* mem) {
     if (mem->run) resident_end(mem->run, false);
     if (mem->eq_tabs) mem->ctx->dev_free(mem->eq_tabs);
     sources_release(mem);
+    rw_release(mem);
+    delete mem->rw;
     for (auto& t : mem->tables) mem->ctx->release(t);
     delete mem;
 }

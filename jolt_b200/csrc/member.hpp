@@ -153,7 +153,10 @@ struct jb_member {
     // product member over sources (jb_member_create_product_sources): the product of its m tables / sources, m <= 16
     // (terms = 1), through product_round_kernel; src as for the expression member over sources
     bool product = false;
-    int ntables() const { return expr ? ex.ntables : m * terms; }
+    // read-write checking member (jb_member_create_read_write): the sparse cycle phase until the last cycle variable is
+    // bound, then an expression member over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (expr set, rw released)
+    struct RwState* rw = nullptr;
+    int ntables() const { return rw ? (int)tables.size() : expr ? ex.ntables : m * terms; }
 };
 
 // The split-eq weight tables of a round (e_out[y >> in_bits] * e_in[y & mask]).
@@ -162,6 +165,42 @@ struct EqWeights {
     const uint64_t* e_in;
     int in_bits;
 };
+
+// read_write.cu ----------------------------------------------------------------------------------------------
+constexpr int RW_MAX_ACCESSES = JB_RW_MAX_ACCESSES;
+// The cycle phase of a read-write checking member: the bound K x T matrix as entries sorted by (row, key), in two
+// buffers that take turns as the input and the output of a bind. Per entry and buffer: key and row (u32), the field
+// arrays ra_0 .. ra_{A-1}, val, vs (Val before the row's block of cycles) and ve (Val after it).
+struct RwState {
+    int A = 0, w = 0;
+    uint64_t coeff[RW_MAX_ACCESSES][4];
+    int d[RW_MAX_ACCESSES];
+    size_t T = 0, K = 0;
+    size_t rows = 0;  // rows of the bound matrix (T >> cycle variables bound)
+    size_t n = 0;     // live entries
+    size_t cap = 0;   // entries a buffer holds: min(K, distinct address columns) * T, which no bind exceeds
+    int cur = 0;      // the buffer holding the current matrix
+    uint32_t* key[2] = {nullptr, nullptr};
+    uint32_t* row[2] = {nullptr, nullptr};
+    uint64_t* f[2] = {nullptr, nullptr};    // (A + 3) x cap field elements
+    uint32_t* off[2] = {nullptr, nullptr};  // row offsets, rows + 1
+    uint32_t* flag = nullptr;               // cap + 1: the scan input
+    uint32_t* base = nullptr;               // cap + 1: the scan output
+    void* scan_tmp = nullptr;
+    size_t scan_bytes = 0;
+    Table inc;                 // inc(j) over the rows, bound alongside
+    uint64_t* init = nullptr;  // K initial values
+};
+// Checks and builds a read-write member without its eq factor (eq_setup adds it); nothing stays allocated on failure.
+int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_kind, int addr_on_device, size_t T,
+              size_t K, const jb_source* inc, const jb_source* init, const uint64_t* w_cycle, size_t nvars,
+              const uint64_t* scale, int order, jb_member** out);
+// One cycle round: binds `bind` (if given), then the pass that leaves q(0), q(inf) in result slot ro.
+int rw_cycle_round(jb_member* mem, const uint64_t* bind, const EqWeights& eqw, jb::RoundOut ro);
+// Binds one cycle variable; after the last one the remaining row is scattered into the member's K-entry tables and
+// the cycle-phase buffers are released.
+int rw_cycle_bind(jb_member* mem, const uint64_t r[4]);
+void rw_release(jb_member* mem);
 
 // product.cu -------------------------------------------------------------------------------------------------
 // One round of a product member: in / out are the member's m table pointers as member_round prepared them (null in
