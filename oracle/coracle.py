@@ -129,6 +129,15 @@ def g1_powers(n: int, g_xy: np.ndarray, beta_mont: np.ndarray) -> np.ndarray:
     return out
 
 
+def g1_powers_fast(n: int, g_xy: np.ndarray, tau_mont: np.ndarray, threads: int | None = None) -> np.ndarray:
+    """The same affine powers tau^i * g as g1_powers, from a fixed-base table of g on all host threads."""
+    out = np.empty((n, 8), dtype=np.uint64)
+    lib().orc_g1_powers_fast(_p(out), ctypes.c_size_t(n), _p(np.ascontiguousarray(g_xy, dtype=np.uint64)),
+                             _p(np.ascontiguousarray(tau_mont, dtype=np.uint64)),
+                             max_threads() if threads is None else threads)
+    return out
+
+
 def g1_msm_naive(bases_xy: np.ndarray, scalars_mont: np.ndarray):
     bases_xy = np.ascontiguousarray(bases_xy, dtype=np.uint64).reshape(-1, 8)
     scalars_mont = np.ascontiguousarray(scalars_mont, dtype=np.uint64).reshape(-1, 4)

@@ -433,6 +433,105 @@ void orc_g1_powers(u64 *out_xy, size_t n, const u64 g_xy[8], const u64 beta_mont
     }
 }
 
+/* The same powers, fast enough for 2^24 points: tau^i on the host, then each tau^i * g as a sum of
+ * one precomputed multiple per c-bit window of tau^i (a fixed-base table of g: table[w][d - 1] =
+ * d * 2^(c w) * g, affine), mixed additions in parallel, and one inversion per chunk of points
+ * (Montgomery's batch trick) back to affine. Identity points (tau = 0) come out as x = y = 0. */
+#define POW_CHUNK 1024
+
+/* Jacobian -> affine for m points with one inversion; identities (Z = 0) become x = y = 0. */
+static void jac_batch_to_affine(u64 *out_xy, const jac_t *p, size_t m, u64 (*scratch)[4]) {
+    u64 acc[4];
+    memcpy(acc, FQ.r1, 32);
+    for (size_t i = 0; i < m; ++i) {  /* scratch[i] = prod of the non-zero Z's before i */
+        memcpy(scratch[i], acc, 32);
+        if (!jac_is_inf(&p[i])) f_mul(&FQ, acc, acc, p[i].z);
+    }
+    u64 inv[4];
+    f_inv(&FQ, inv, acc);
+    for (size_t i = m; i-- > 0;) {
+        if (jac_is_inf(&p[i])) { memset(out_xy + 8 * i, 0, 64); continue; }
+        u64 zi[4], zi2[4], zi3[4];
+        f_mul(&FQ, zi, inv, scratch[i]);
+        f_mul(&FQ, inv, inv, p[i].z);
+        f_mul(&FQ, zi2, zi, zi);
+        f_mul(&FQ, zi3, zi2, zi);
+        f_mul(&FQ, out_xy + 8 * i, p[i].x, zi2);
+        f_mul(&FQ, out_xy + 8 * i + 4, p[i].y, zi3);
+    }
+}
+
+static u64 window_digit(const u64 k[4], int bit, int c) {
+    int limb = bit / 64, off = bit % 64;
+    u64 d = k[limb] >> off;
+    if (off + c > 64 && limb < 3) d |= k[limb + 1] << (64 - off);
+    return d & (((u64)1 << c) - 1);
+}
+
+void orc_g1_powers_fast(u64 *out_xy, size_t n, const u64 g_xy[8], const u64 tau_mont[4], int threads) {
+    if (n == 0) return;
+    const int nt = threads > 1 ? threads : 1;
+    const int c = n >= ((size_t)1 << 16) ? 16 : 8;
+    const int nwin = (254 + c - 1) / c;
+    const size_t nd = ((size_t)1 << c) - 1;
+    /* the table: window w starts from 2^(c w) * g and adds it nd - 1 times */
+    u64 *table = (u64 *)malloc((size_t)nwin * nd * 64);
+    jac_t base;
+    jac_set_inf(&base); memset(base.z, 0, 32);
+    jac_add_affine(&base, &base, g_xy, g_xy + 4);
+    u64 *bases = (u64 *)malloc((size_t)nwin * 64);
+    for (int w = 0; w < nwin; ++w) {
+        jac_to_affine(bases + 8 * w, &base);
+        for (int k = 0; k < c; ++k) jac_double(&base, &base);
+    }
+#pragma omp parallel for schedule(dynamic, 1) num_threads(nt)
+    for (size_t job = 0; job < (size_t)nwin * ((nd + POW_CHUNK - 1) / POW_CHUNK); ++job) {
+        const size_t per = (nd + POW_CHUNK - 1) / POW_CHUNK;
+        const int w = (int)(job / per);
+        const size_t lo = (job % per) * POW_CHUNK, hi = lo + POW_CHUNK < nd ? lo + POW_CHUNK : nd;
+        const u64 *b = bases + 8 * w;
+        jac_t *pts = (jac_t *)malloc(sizeof(jac_t) * POW_CHUNK);
+        u64(*scratch)[4] = malloc(32 * POW_CHUNK);
+        u64 k[4] = {lo + 1, 0, 0, 0}, km[4];
+        orc_f_to_mont(0, km, k);
+        jac_scalar_mul_affine(&pts[0], b, k);  /* (lo + 1) * b, then + b per entry */
+        for (size_t d = lo + 1; d < hi; ++d) jac_add_affine(&pts[d - lo], &pts[d - lo - 1], b, b + 4);
+        jac_batch_to_affine(table + ((size_t)w * nd + lo) * 8, pts, hi - lo, scratch);
+        free(scratch);
+        free(pts);
+    }
+    free(bases);
+    /* tau^i: the first power of each chunk by exponentiation, the rest by one multiplication each */
+    u64 tau[4];
+    memcpy(tau, tau_mont, 32);
+#pragma omp parallel for schedule(dynamic, 1) num_threads(nt)
+    for (size_t lo = 0; lo < n; lo += POW_CHUNK) {
+        const size_t hi = lo + POW_CHUNK < n ? lo + POW_CHUNK : n;
+        jac_t *pts = (jac_t *)malloc(sizeof(jac_t) * POW_CHUNK);
+        u64(*scratch)[4] = malloc(32 * POW_CHUNK);
+        u64 e[4] = {lo, 0, 0, 0}, pw[4];
+        f_pow(&FR, pw, tau, e);
+        for (size_t i = lo; i < hi; ++i) {
+            u64 k[4];
+            orc_f_from_mont(0, k, pw);
+            jac_t *acc = &pts[i - lo];
+            jac_set_inf(acc); memset(acc->z, 0, 32);
+            for (int w = 0; w < nwin; ++w) {
+                const u64 d = window_digit(k, w * c, c);
+                if (d) {
+                    const u64 *t = table + ((size_t)w * nd + d - 1) * 8;
+                    jac_add_affine(acc, acc, t, t + 4);
+                }
+            }
+            f_mul(&FR, pw, pw, tau);
+        }
+        jac_batch_to_affine(out_xy + 8 * lo, pts, hi - lo, scratch);
+        free(scratch);
+        free(pts);
+    }
+    free(table);
+}
+
 /* naive MSM: sum_i s_i * P_i (jolt-crypto/tests/group_laws.rs:69-79). */
 int orc_g1_msm_naive(u64 out_xy[8], const u64 *bases_xy, const u64 *scalars_mont, size_t n) {
     jac_t acc;

@@ -1,6 +1,7 @@
 """HyperKZG prover side on the device vs the oracle (mirrors crates/jolt-hyperkzg/src/scheme.rs:382-417,
-tests/commit_open_verify.rs:50-188 on the prover side; the pairing check itself is out of scope).
-G1 results are compared as affine (x, y) integers (parity unpinned by golden vectors)."""
+tests/commit_open_verify.rs:50-188 on the prover side), every proof also checked by the reference verifier
+(tests/hyperkzg_ref.py) over a power SRS whose secret the test knows. G1 results are compared as affine (x, y)
+integers."""
 import numpy as np
 import pytest
 
@@ -9,6 +10,7 @@ from jolt_b200 import G1Bases, HyperKZG, Polynomial, g1_jacobian_to_affine
 from jolt_b200 import field as F
 from oracle import bn254 as O
 from oracle import coracle as C
+import hyperkzg_ref as HK
 from gpu_util import rand_challenge, rand_limbs
 
 pytestmark = pytest.mark.gpu
@@ -23,45 +25,14 @@ def sess():
     s.close()
 
 
-def oracle_affine(xy, inf):
-    return None if inf else (O.from_mont_limbs(xy[:4], O.Q_MOD), O.from_mont_limbs(xy[4:], O.Q_MOD))
-
-
-def oracle_open(srs_xy, evals_limbs, point_limbs, r_int, q_int):
-    """scheme.rs:122-158 + kzg.rs:69-126 with the C oracle doing the table-sized work."""
-    thr = C.max_threads()
-    ell = point_limbs.shape[0]
-    polys = [evals_limbs]
-    for i in range(1, ell):
-        polys.append(C.bind(polys[-1], point_limbs[ell - i], O.LOW_TO_HIGH, thr))
-    com = [oracle_affine(*C.g1_msm_pippenger(srs_xy[: p.shape[0]], p, 0, thr)) for p in polys[1:]]
-    u = [r_int % O.R_MOD, (-r_int) % O.R_MOD, r_int * r_int % O.R_MOD]
-    v = [[C.mont_to_ints(C.eval_univariate(p, C.ints_to_mont([ui])[0]))[0] for p in polys] for ui in u]
-    n = evals_limbs.shape[0]
-    b = np.zeros((n, 4), dtype=np.uint64)
-    qj = 1
-    for p in polys:
-        scaled = C.f_vec(0, 2, p, np.tile(C.ints_to_mont([qj]), (p.shape[0], 1)))
-        b[: p.shape[0]] = C.f_vec(0, 0, b[: p.shape[0]], scaled)
-        qj = qj * q_int % O.R_MOD
-    w = []
-    for ui in u:
-        h = C.witness_polynomial(b, C.ints_to_mont([ui])[0])
-        w.append(oracle_affine(*C.g1_msm_pippenger(srs_xy[: h.shape[0]], h, 0, thr)) if h.shape[0] else None)
-    return com, w, v
-
-
 @pytest.mark.parametrize("ell,precompute", [(1, False), (2, False), (3, True), (5, False), (8, True), (11, False),
                                             (14, False), (14, True), (4, True), (16, True), (17, True)])
 def test_open_matches_oracle(sess, ell, precompute):
     n = 1 << ell
-    beta = C.ints_to_mont([O.random_fr(0x4D534D, 1)[0]])[0]
-    srs_xy = C.g1_powers(n, G, beta) if ell <= 11 else None
-    if srs_xy is None:      # big SRS: sequential multiples generated on the device (any valid bases do)
-        bases = G1Bases.generate_multiples(sess, G, n)
-        srs_xy = bases.affine()
-    else:
-        bases = G1Bases.from_affine(sess, srs_xy)
+    tau = O.random_fr(0x4D534D, 1)[0]
+    beta = C.ints_to_mont([tau])[0]
+    srs_xy = C.g1_powers(n, G, beta) if ell <= 11 else C.g1_powers_fast(n, G, beta)
+    bases = G1Bases.from_affine(sess, srs_xy)
     if precompute:       # fixed-SRS tables: shared buckets for the large MSMs, the 8-bit table for the small ones
         bases.precompute()
     evals = rand_limbs(100 + ell, n)
@@ -79,19 +50,22 @@ def test_open_matches_oracle(sess, ell, precompute):
 
     poly = Polynomial.new(sess, evals)
     commitment = g1_jacobian_to_affine(HyperKZG.commit(bases, poly))
-    assert commitment == oracle_affine(*C.g1_msm_pippenger(srs_xy, evals, 0, C.max_threads()))
+    assert commitment == HK.oracle_affine(*C.g1_msm_pippenger(srs_xy, evals, 0, C.max_threads()))
     proof = HyperKZG.open(bases, poly, point, ch_r, ch_q)
-    com, w, v = oracle_open(srs_xy, evals, point, r_int, q_int)
+    com, w, v = HK.oracle_open(srs_xy, evals, point, r_int, q_int)
     assert seen["com"] == com and [g1_jacobian_to_affine(c) for c in proof.com] == com
     assert proof.v == v and seen["v"] == v
     assert [g1_jacobian_to_affine(x) for x in proof.w] == w
     # the table is untouched by open (the reference borrows `evals`)
     assert (poly.evals() == evals).all()
-    # HyperKZG consistency (what the verifier's first check enforces): folding the last polynomial with
-    # point[0] gives the multilinear evaluation; and v[0][j], v[1][j] determine v[2][j+1] (scheme.rs:200-230)
+    # the proof verifies for y = the multilinear evaluation at the point, and not for any other y
+    y = HK.host_eval(evals, point)
     if ell <= 8:
-        pt_int = F.limbs_to_ints(point)
-        assert O.evaluate(C.mont_to_ints(evals), pt_int) is not None
+        assert y == O.evaluate(C.mont_to_ints(evals), F.limbs_to_ints(point))
+    pt = F.limbs_to_ints(point)
+    d0 = O.random_fr(2000 + ell, 1)[0]
+    assert HK.verify(tau, commitment, pt, y, com, w, v, r_int, q_int, d0)
+    assert not HK.verify(tau, commitment, pt, (y + 1) % O.R_MOD, com, w, v, r_int, q_int, d0)
 
 
 def test_open_rejects_bad_input(sess):
