@@ -318,6 +318,38 @@ int jb_member_create_read_write(jb_ctx* ctx, const jb_rw_access* accesses, size_
                                 int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
                                 const jb_source* init, const uint64_t* w_cycle, size_t nvars, const uint64_t* scale_or_null,
                                 int order, jb_member** out);
+/* Booleanity member (Shout's booleanity check on the RA polynomials): ProveRounds for
+ *   sum_{k<K} sum_{j<T} scale * eq(r_addr, k) * eq(r_cycle, j) * sum_{i<d} c_i * (ra_i(k, j)^2 - ra_i(k, j)),
+ *   ra_i(k, j) = [addr_i(j) = k]   (0 where addr_i(j) is the none value),
+ * over the whole K x T matrix from the d = count address columns, holding O(d * T + d * K) memory and never K * T.
+ *  - Columns: count (1 <= count <= JB_BOOL_MAX_POLYS) address columns of T entries of one `kind` (JB_SCALAR_U8 / U16;
+ *    the none value and the address rules are jb_one_hot_evaluate's), all in host memory or all in caller-owned device
+ *    memory (on_device), aligned to their entry, borrowed for the call. K and T are powers of two, K <= 2^16,
+ *    T < 2^31, K * T >= 2. coeffs: count x 4 canonical limbs (c_i). r_addr: log2 K and r_cycle: log2 T canonical
+ *    coordinates, r_addr[0] and r_cycle[0] <-> the most significant bits; optional scale.
+ *  - Variables: the log2 K address bits first, then the log2 T cycle bits; `order` applies within each phase.
+ *    JB_HIGH_TO_LOW binds the address MSB first, then the cycle MSB first: HighToLow over the address-major index
+ *    x = k * T + j with eq point r_addr || r_cycle. JB_LOW_TO_HIGH binds the address LSB first, then the cycle LSB
+ *    first: LowToHigh over the cycle-major index x = j * K + k with eq point r_cycle || r_addr. Each order's rounds are
+ *    bit-identical to jb_member_create_expr over the materialised ra tables in that layout.
+ *  - degree 3; log2 K + log2 T rounds; the running claim is mandatory in prove_round. A zero eq factor at the current
+ *    variable is refused, as in jb_eq_member_create. The address rounds work on K-entry tables from the pushforward
+ *    (G_i, bound linearly, and a copy Q_i bound by the squared rule (1-r)^2 lo + r^2 hi); the cycle rounds gather
+ *    F[addr_i(j)], F = eq(rho_addr, .), from the columns in their first two rounds and then bind d field tables of
+ *    T / 2 entries.
+ *  - jb_member_final_evals returns ra_0 .. ra_{d-1} at the bound point, in column order. jb_eq_member_scalar returns
+ *    scale * eq(r_addr, rho_addr) * eq(r_cycle, rho_cycle) after the rounds.
+ *  - Everything the rounds need is allocated at creation, so JB_ERR_OOM can only arise here.
+ * Errors, checked before anything is allocated: JB_ERR_INVALID for a null pointer, count 0, an unknown kind or order,
+ * a bad T or K, a non-canonical coefficient, point or scale, on_device not 0 / 1 or a misaligned device column;
+ * JB_ERR_UNSUPPORTED for count > JB_BOOL_MAX_POLYS or T >= 2^31. An address >= K that is not the none value is found on
+ * the device at creation: JB_ERR_INVALID, with nothing left allocated. The member works in jb_prove_batch and
+ * jb_scheduler_*; it never runs in a resident kernel and is not sharded (jb_member_prove_round_partials returns
+ * JB_ERR_UNSUPPORTED). */
+#define JB_BOOL_MAX_POLYS 32
+int jb_member_create_booleanity(jb_ctx* ctx, const void* const* columns, size_t count, int kind, int on_device,
+                                size_t T, size_t K, const uint64_t* coeffs, const uint64_t* r_addr,
+                                const uint64_t* r_cycle, const uint64_t* scale_or_null, int order, jb_member** out);
 /* Multi-GPU: like prove_round but leaves this rank's partial sums - the kernel values s(0), [s(1) unless
  * skip_t1], s(2), .., s(m-1), s(inf) in the order jb_round_evals_from_kernel_values documents - on the device as
  * count x 8 uint64 lanes, each holding one 32-bit limb (exact under ncclSum over <= 2^32 ranks); the caller

@@ -31,6 +31,7 @@ from .api import (  # noqa: F401
     ProductSourcesMember,
     ProvedBatch,
     ReadWriteCheckingMember,
+    BooleanityMember,
     RoundScheduler,
     Session,
     SumOfProductsMember,

@@ -67,6 +67,9 @@ SIGNATURES = {
     "jb_member_create_read_write": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, ctypes.c_int, ctypes.c_int,
                                                    c_size_t, c_size_t, c_void_p, c_void_p, c_u64p, c_size_t, c_u64p,
                                                    ctypes.c_int, ctypes.POINTER(c_void_p)]),
+    "jb_member_create_booleanity": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, ctypes.c_int,
+                                                   c_size_t, c_size_t, c_u64p, c_u64p, c_u64p, c_u64p, ctypes.c_int,
+                                                   ctypes.POINTER(c_void_p)]),
     "jb_member_prove_round_partials": (ctypes.c_int, [c_void_p, c_u64p, c_size_t, ctypes.c_int, c_void_p]),
     "jb_ctx_set_verify_rounds": (ctypes.c_int, [c_void_p, ctypes.c_int]),
     "jb_partials_finalize": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_u64p]),
@@ -163,6 +166,7 @@ class SourceC(ctypes.Structure):
 
 
 JB_RW_MAX_ACCESSES = 4
+JB_BOOL_MAX_POLYS = 32
 
 
 class RwAccessC(ctypes.Structure):

@@ -906,6 +906,39 @@ class ReadWriteCheckingMember(ExpressionMember):
         self.m = 3
 
 
+class BooleanityMember(ExpressionMember):
+    """Shout booleanity of the RA polynomials (jb_member_create_booleanity): ProveRounds for
+      sum_{k<K} sum_{j<T} scale * eq(r_addr, k) * eq(r_cycle, j) * sum_i c_i * (ra_i(k, j)^2 - ra_i(k, j))
+    with ra_i(k, j) = [columns[i][j] = k], from up to 32 uint8 / uint16 address columns (numpy arrays or CUDA tensors
+    of one dtype and length T; the all-ones value = no address), in O(d T + d K) memory. `coeffs`: one c_i per column
+    (an int or 4 Montgomery limbs); r_addr (log2 K) and r_cycle (log2 T) coordinates, [0] <-> the MSB. The address
+    variables are bound first, then the cycle variables; HIGH_TO_LOW binds each phase MSB first (address-major index
+    k T + j, eq point r_addr || r_cycle), LOW_TO_HIGH LSB first (cycle-major index j K + k, eq point r_cycle || r_addr).
+    Degree 3, log2 K + log2 T rounds; the running claim is mandatory. final_evals() returns ra_0 .. ra_{d-1} at the
+    bound point; eq_scalar() returns scale * eq(r_addr, rho_addr) * eq(r_cycle, rho_cycle)."""
+
+    def __init__(self, session: Session, columns, K: int, coeffs, r_addr, r_cycle, scale=None,
+                 order: int = LOW_TO_HIGH):
+        ptrs, kind, T, dev, _keep = _address_columns(columns, "BooleanityMember")
+        if len(coeffs) != len(ptrs):
+            raise ValueError("BooleanityMember: one coefficient per column")
+        cf = np.zeros((max(len(ptrs), 1), 4), dtype=np.uint64)
+        for i, c in enumerate(coeffs):
+            cf[i] = _limbs(c % F.R_MOD if isinstance(c, (int, np.integer)) else c)
+        ra, rc = point_limbs(r_addr), point_limbs(r_cycle)
+        sc = None if scale is None else _limbs(scale)
+        h = ctypes.c_void_p()
+        session.check(session.lib.jb_member_create_booleanity(
+            session.h, (ctypes.c_void_p * max(len(ptrs), 1))(*ptrs), len(ptrs), kind, dev, T, K, _p(cf),
+            _p(ra) if ra.shape[0] else None, _p(rc) if rc.shape[0] else None, _p(sc) if sc is not None else None, order,
+            ctypes.byref(h)))
+        self.s = session
+        self.h = h
+        self.ntables = len(ptrs)
+        self._degree = 3
+        self.m = 3
+
+
 def _monomials_c(monomials):
     mons = (_lib.MonomialC * max(len(monomials), 1))()
     for k, (coeff, tabs) in enumerate(monomials):

@@ -219,7 +219,7 @@ jb_ctx* jb_member_context(jb_member* mem) { return mem ? mem->ctx : nullptr; }
 
 int jb_member_num_tables(jb_member* mem, size_t* tables) {
     if (!mem || !tables) return JB_ERR_INVALID;
-    *tables = (size_t)mem->ntables();
+    *tables = mem->bl ? (size_t)mem->bl->d : (size_t)mem->ntables();
     return JB_OK;
 }
 
@@ -672,20 +672,35 @@ int jb_member_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
 
 // ---- split-eq member: one round ------------------------------------------------------------------------
 // scalar <- scalar * eq(w_v, r) for the variable v just bound (GruenSplitEqPolynomial::bind, split_eq.rs:347-352)
-static void eq_absorb_bind(jb_member* mem, size_t var, const uint64_t* r) {
-    HostFr wv = HostFr::from_limbs(mem->eq_w.data() + 4 * var), rr = HostFr::from_limbs(r);
+static void eq_absorb_coord(jb_member* mem, const uint64_t* w, const uint64_t* r) {
+    HostFr wv = HostFr::from_limbs(w), rr = HostFr::from_limbs(r);
     HostFr prod = wv * rr;
     HostFr f = HostFr::one() - wv - rr + prod + prod;
     (HostFr::from_limbs(mem->eq_scalar) * f).store(mem->eq_scalar);
 }
+static void eq_absorb_bind(jb_member* mem, size_t var, const uint64_t* r) { eq_absorb_coord(mem, mem->eq_w.data() + 4 * var, r); }
 
 static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
+static int bool_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
+static int eq_round_tail(jb_member* mem, const HostFr& l0, const HostFr& l1, const uint64_t* claim, size_t round,
+                         uint64_t* out_evals);
 
 static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
     jb_ctx* c = mem->ctx;
     if (!claim) return c->fail(JB_ERR_INVALID, "eq member: the running claim is required (Gruen hint s(0)+s(1))");
-    const size_t n = mem->eq_n, M = (size_t)mem->m;
+    const size_t n = mem->eq_n;
     if (mem->rw && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
+    if (mem->bl) {  // the address rounds come first; the cycle rounds are this member's eq rounds
+        const size_t ka = mem->bl->log_k;
+        if (round < ka) return bool_address_round(mem, bind, round, claim, out_evals);
+        if (round == ka && bind) {  // the last address variable
+            eq_absorb_coord(mem, bool_addr_coord(*mem->bl, ka - 1), bind);
+            const int st = bool_begin_cycles(mem, bind);
+            if (st != JB_OK) return st;
+            bind = nullptr;
+        }
+        round -= ka;
+    }
     if (round >= n) return c->fail(JB_ERR_INVALID, "prove_round: member is fully bound");
     const bool l2h = mem->order == JB_LOW_TO_HIGH;
     if (bind) {
@@ -721,14 +736,24 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     const HostFr wc = HostFr::from_limbs(mem->eq_w.data() + 4 * cur_var);
     const HostFr l1 = scalar * wc, l0 = scalar - l1;
     if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
-    int st = mem->rw ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
-                     : member_round(mem, bind, true, nullptr, &er);
+    int st = mem->rw   ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+             : mem->bl ? bool_cycle_pass(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+                       : member_round(mem, bind, true, nullptr, &er);
     if (st != JB_OK) return st;
+    return eq_round_tail(mem, l0, l1, claim, round, out_evals);
+}
+
+// The host half of a split-eq round whose pass is in flight: waits for q(0), q(2) .. q(M-1), q(inf) in result slot 0,
+// takes q(1) from the claim, s(t) = l(t) q(t) for t = 0 .. M + 1 with l(t) = l0 + t (l1 - l0) (l1 invertible).
+static int eq_round_tail(jb_member* mem, const HostFr& l0, const HostFr& l1, const uint64_t* claim, size_t round,
+                         uint64_t* out_evals) {
+    jb_ctx* c = mem->ctx;
+    const size_t M = (size_t)mem->m;
     // a field inversion is ~400 host multiplications (~13 us): do it while the device runs the pass (the
     // extrapolation constants below are built once)
     const HostFr l1_inv = l1.inverse();
     const RoundConsts& rc = round_consts((int)M);
-    st = wait_round_result0(c);
+    int st = wait_round_result0(c);
     if (st != JB_OK) return st;
     // kernel order: q(0), q(2), .., q(M-1), q(inf)   (M <= 16 values; q(0) only for M == 1)
     const HostFr q0 = HostFr::from_limbs(c->h_result);
@@ -1146,6 +1171,39 @@ int jb_member_create_read_write(jb_ctx* c, const jb_rw_access* accesses, size_t 
     return eq_setup(mem, w_cycle, nvars, scale_or_null, out);
 }
 
+// ---- booleanity member ----------------------------------------------------------------------------------
+// An address round: the address coordinate of the previous round is absorbed into the eq scalar, the current one's
+// factor l(t) is the host's, and the pass over the K-entry tables (which binds the previous variable) gives q.
+static int bool_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
+    jb_ctx* c = mem->ctx;
+    const BoolState& bl = *mem->bl;
+    if (bind) eq_absorb_coord(mem, bool_addr_coord(bl, round - 1), bind);
+    const HostFr scalar = HostFr::from_limbs(mem->eq_scalar);
+    const HostFr l1 = scalar * HostFr::from_limbs(bool_addr_coord(bl, round)), l0 = scalar - l1;
+    if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
+    const int st = bool_address_pass(mem, bind, round, round_out(c, nullptr, 0, nullptr));
+    if (st != JB_OK) return st;
+    return eq_round_tail(mem, l0, l1, claim, round, out_evals);
+}
+
+int jb_member_create_booleanity(jb_ctx* c, const void* const* columns, size_t count, int kind, int on_device, size_t T,
+                                size_t K, const uint64_t* coeffs, const uint64_t* r_addr, const uint64_t* r_cycle,
+                                const uint64_t* scale_or_null, int order, jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    jb_member* mem = nullptr;
+    {
+        Guard g(c);
+        const int st = bool_create(c, columns, count, kind, on_device, T, K, coeffs, r_addr, r_cycle, scale_or_null,
+                                   order, &mem);
+        if (st != JB_OK) return st;
+    }
+    *out = mem;
+    if (T >= 2) return eq_setup(mem, r_cycle, mem->bl->log_t, scale_or_null, out);
+    mem->eq = true;  // T = 1: address rounds only, no cycle eq tables
+    (scale_or_null ? HostFr::from_limbs(scale_or_null) : HostFr::one()).store(mem->eq_scalar);
+    return JB_OK;
+}
+
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
 int jb_eq_member_scalar(jb_member* mem, uint64_t out[4]) {
     if (!mem || !out || !mem->eq) return JB_ERR_INVALID;
@@ -1316,6 +1374,7 @@ int jb_member_prove_round_partials(jb_member* mem, const uint64_t* bind, size_t 
     if (mem->expr) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: expression members are not sharded");
     if (mem->product) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: product members are not sharded");
     if (mem->rw) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: read-write members are not sharded");
+    if (mem->bl) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: booleanity members are not sharded");
     before_launch(mem);
     return member_round(mem, bind, skip_t1 != 0, lanes_out);
 }
@@ -1424,6 +1483,7 @@ int jb_member_export_table(jb_member* mem, size_t j, void* device_dst, size_t ca
     jb_ctx* c = mem->ctx;
     Guard g(c, true);
     before_launch(mem);  // the host's view of the tables (buffer parity, length) is exact at a round boundary
+    if (mem->bl) return c->fail(JB_ERR_INVALID, "export_table: a booleanity member keeps its tables to itself");
     if (j >= (size_t)mem->ntables()) return c->fail(JB_ERR_INVALID, "export_table: table index out of range");
     if (mem->rw && !mem->expr) return c->fail(JB_ERR_INVALID, "export_table: a read-write member in its cycle rounds has no tables");
     if (!mem->src.empty() && mem->src[j].type != JB_SOURCE_TABLE)
@@ -1448,6 +1508,16 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
         if (mem->len != 2) return c->fail(JB_ERR_INVALID, "finish_rounds: rounds remain");
         eq_absorb_bind(mem, 0, bind);
         return rw_bind_cycle(mem, bind);
+    }
+    if (mem->bl) {  // the last variable: a cycle variable, or the last address variable when T = 1
+        if (mem->len != 2) return c->fail(JB_ERR_INVALID, "finish_rounds: rounds remain");
+        const BoolState& bl = *mem->bl;
+        eq_absorb_coord(mem, bl.T == 1 ? bool_addr_coord(bl, bl.log_k - 1)
+                                       : mem->eq_w.data() + 4 * (mem->order == JB_LOW_TO_HIGH ? 0 : mem->eq_n - 1), bind);
+        before_launch(mem);
+        const int st = bool_finish(mem, bind);
+        if (st == JB_OK) mem->len = 1;
+        return st;
     }
     if (mem->eq && !mem->rw) {
         size_t var = 0;
@@ -1476,8 +1546,11 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     return JB_OK;
 }
 
+static int bool_final_evals(jb_member* mem, uint64_t* out);
+
 int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     if (!mem || !out) return JB_ERR_INVALID;
+    if (mem->bl) return bool_final_evals(mem, out);
     jb_ctx* c = mem->ctx;
     if (mem->sharded && !mem->gathered) {
         if (!mem->tail) return c->fail(JB_ERR_INVALID, "NotFullyBound (sharded member before its tail)");
@@ -1508,6 +1581,30 @@ int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     return JB_OK;
 }
 
+// ra_0 .. ra_{d-1} of a fully bound booleanity member
+static int bool_final_evals(jb_member* mem, uint64_t* out) {
+    jb_ctx* c = mem->ctx;
+    Guard g(c, true);
+    if (mem->len != 1) {
+        char buf[96];
+        size_t remaining = 0;
+        for (size_t l = mem->len; l > 1; l >>= 1) ++remaining;
+        std::snprintf(buf, sizeof buf, "NotFullyBound { remaining: %zu }", remaining);
+        return c->fail(JB_ERR_INVALID, buf);
+    }
+    before_launch(mem);
+    const int d = mem->bl->d;
+    for (int j = 0; j < d; ++j) {
+        int st = c->check(cudaMemcpyAsync(c->h_small + 4 * j, bool_final_entry(mem, j), 32, cudaMemcpyDeviceToHost, c->stream),
+                          "final evals D2H");
+        if (st != JB_OK) return st;
+    }
+    int st = c->check(cudaStreamSynchronize(c->stream), "final evals sync");
+    if (st != JB_OK) return st;
+    std::memcpy(out, c->h_small, (size_t)d * 32);
+    return JB_OK;
+}
+
 void jb_member_destroy(jb_member* mem) {
     if (!mem) return;
     if (mem->tail) jb_member_destroy(mem->tail);
@@ -1517,6 +1614,8 @@ void jb_member_destroy(jb_member* mem) {
     sources_release(mem);
     rw_release(mem);
     delete mem->rw;
+    bool_release(mem);
+    delete mem->bl;
     for (auto& t : mem->tables) mem->ctx->release(t);
     delete mem;
 }

@@ -157,6 +157,9 @@ struct jb_member {
     // bound, then an expression member over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (expr set, rw released)
     struct RwState* rw = nullptr;
     int ntables() const { return rw ? (int)tables.size() : expr ? ex.ntables : m * terms; }
+    // booleanity member (jb_member_create_booleanity): its d tables live in bl, not in `tables`, and ntables() does not
+    // count them (the entry points that report or read tables ask bl for d)
+    struct BoolState* bl = nullptr;
 };
 
 // The split-eq weight tables of a round (e_out[y >> in_bits] * e_in[y & mask]).
@@ -201,6 +204,57 @@ int rw_cycle_round(jb_member* mem, const uint64_t* bind, const EqWeights& eqw, j
 // the cycle-phase buffers are released.
 int rw_cycle_bind(jb_member* mem, const uint64_t r[4]);
 void rw_release(jb_member* mem);
+
+// booleanity.cu ----------------------------------------------------------------------------------------------
+constexpr int BOOL_MAX_POLYS = JB_BOOL_MAX_POLYS;
+// The state of a booleanity member. Address phase: G_i (bound linearly) and Q_i (bound by the squared rule) as d
+// tables packed at the current length in gq[cur] (G then Q), the other buffer receiving the next bind; eq_rest holds
+// eq over the address coordinates after the current one, one table per address round. Cycle phase: F = eq(rho_addr, .)
+// and the member's copy of the columns until cycle round 1 binds them into h[0] (d tables at stride T / 2);
+// LowToHigh binds alternate between h[0] and h[1] (stride T / 4), HighToLow binds h[0] in place.
+struct BoolState {
+    int d = 0, kind = 0, order = 0;
+    size_t T = 0, K = 0, log_k = 0, log_t = 0;
+    uint64_t coeff[BOOL_MAX_POLYS][4];
+    std::vector<uint64_t> r_addr;  // log_k coordinates, r_addr[0] <-> MSB
+    std::vector<uint64_t> rho;     // the address challenges bound so far, in binding order
+    size_t klen = 0;               // address phase: current table length (0 once the cycle phase began)
+    int gq_cur = 0;
+    uint64_t* gq[2] = {nullptr, nullptr};  // 2 d K and 2 d K / 2 elements
+    uint64_t* eq_rest = nullptr;           // K - 1 elements: round m's table at K - 2^(log_k - m)
+    uint64_t* F = nullptr;                 // K elements
+    void* cols = nullptr;                  // d x T addresses (member-owned), until cycle round 1
+    size_t hlen = 0;                       // cycle phase: current table length (T while the columns are unbound)
+    int h_cur = 0;
+    uint64_t* h[2] = {nullptr, nullptr};
+    size_t h_stride[2] = {0, 0};
+};
+// Checks and builds a booleanity member without its cycle eq factor (the caller adds it); nothing stays allocated on
+// failure.
+int bool_create(jb_ctx* c, const void* const* columns, size_t count, int kind, int on_device, size_t T, size_t K,
+                const uint64_t* coeffs, const uint64_t* r_addr, const uint64_t* r_cycle, const uint64_t* scale,
+                int order, jb_member** out);
+// The address coordinate that address round m binds.
+const uint64_t* bool_addr_coord(const BoolState& bl, size_t m);
+// Address round m: binds `bind` (if given; the previous address variable) into G and Q, then the pass that leaves
+// q(0), q(inf) in result slot ro.
+int bool_address_pass(jb_member* mem, const uint64_t* bind, size_t m, jb::RoundOut ro);
+// The end of the address phase: rho gets the last address challenge (if any), F = eq(rho_addr, .) is built and the
+// address tables are released.
+int bool_begin_cycles(jb_member* mem, const uint64_t* last_addr_challenge);
+// A cycle round: binds `bind` (if given), then the pass that leaves q(0), q(inf) in result slot ro.
+int bool_cycle_pass(jb_member* mem, const uint64_t* bind, const EqWeights& eqw, jb::RoundOut ro);
+// The terminal bind (two entries per table left): a cycle variable, or the last address variable when T = 1.
+int bool_finish(jb_member* mem, const uint64_t r[4]);
+// Where ra_i's single entry lies once the member is fully bound.
+const uint64_t* bool_final_entry(const jb_member* mem, int i);
+void bool_release(jb_member* mem);
+
+// mle_eval.cu ------------------------------------------------------------------------------------------------
+// G_p[k] = sum_{j: addr_p(j) = k} eq(r_cycle, j) for count device address columns into out[p] (K elements each);
+// JB_ERR_INVALID (fail_bad_address) for an address >= K that is not none. Waits for the device.
+int one_hot_pushforward_into(jb_ctx* c, const void* const* dev_columns, size_t count, int kind, size_t T, size_t K,
+                             const uint64_t* r_cycle, uint64_t* const* out);
 
 // product.cu -------------------------------------------------------------------------------------------------
 // One round of a product member: in / out are the member's m table pointers as member_round prepared them (null in

@@ -270,6 +270,34 @@ int launch_small(EvalPlan& p, int kind, size_t first, size_t n) {
 
 }  // namespace
 
+int one_hot_pushforward_into(jb_ctx* c, const void* const* dev_columns, size_t count, int kind, size_t T, size_t K,
+                             const uint64_t* r_cycle, uint64_t* const* out) {
+    EvalPlan p(c);
+    for (size_t i = 0; i < count; ++i) p.cols.push_back(EvalCol{dev_columns[i], i});
+    int st = p.begin(r_cycle, (size_t)log2_of(T), K * 8);
+    if (st == JB_OK) {
+        const bool sm = K <= PF_SMEM_K;
+#define JB_PF_LAUNCH(KD, SM)                                                                                       \
+    pushforward_kernel<KD, SM><<<p.grid, EV_BLOCK, 0, c->stream>>>(p.d_cols, count, p.e_hi(), p.e_lo(), p.n_lo, p.rows, \
+                                                                    p.rpb, (uint32_t)K, p.d_lanes, p.bad())
+        if (kind == SK_U8) { if (sm) JB_PF_LAUNCH(SK_U8, true); else JB_PF_LAUNCH(SK_U8, false); }
+        else { if (sm) JB_PF_LAUNCH(SK_U16, true); else JB_PF_LAUNCH(SK_U16, false); }
+#undef JB_PF_LAUNCH
+        c->launches++;
+        st = c->check(cudaGetLastError(), "pushforward_kernel launch");
+    }
+    unsigned int flag = 0;
+    if (st == JB_OK) st = c->check(cudaMemcpyAsync(&flag, p.bad(), 4, cudaMemcpyDeviceToHost, c->stream), "pushforward flag D2H");
+    if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "pushforward sync");
+    if (st == JB_OK && flag) st = fail_bad_address(c);
+    for (size_t i = 0; i < count && st == JB_OK; ++i) {
+        bins_to_fr_kernel<<<launch_grid(c, K, BINS_BLOCK, 8), BINS_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, out[i]);
+        c->launches++;
+        st = c->check(cudaGetLastError(), "bins_to_fr_kernel launch");
+    }
+    return st;  // (EvalPlan frees its buffers stream-ordered, after the conversions)
+}
+
 extern "C" {
 
 int jb_table_evaluate_batch(jb_ctx* c, const jb_table* tables, size_t count, const uint64_t* point, size_t nvars,
@@ -376,52 +404,28 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
     if ((st = check_point(c, r_cycle, log_t, "one_hot_pushforward: null point")) != JB_OK) return st;
     if (count == 0) return JB_OK;
     Guard g(c);
-    EvalPlan p(c);
     Columns cols(c);
+    std::vector<const void*> dcols(count, nullptr);
+    for (size_t i = 0; i < count && st == JB_OK; ++i)
+        st = cols.get(columns[i], T * (size_t)small_kind_bytes(kind), on_device, &dcols[i]);
+    // the tables are handed out only once the bins are known to be valid
+    std::vector<Table> made(count);
+    std::vector<uint64_t*> bufs(count, nullptr);
     for (size_t i = 0; i < count && st == JB_OK; ++i) {
-        const void* d = nullptr;
-        st = cols.get(columns[i], T * (size_t)small_kind_bytes(kind), on_device, &d);
-        p.cols.push_back(EvalCol{d, i});
+        st = c->dev_alloc((void**)&made[i].buf, K * 32);
+        made[i].cap = made[i].len = K;
+        bufs[i] = made[i].buf;
     }
-    if (st == JB_OK) st = p.begin(r_cycle, log_t, K * 8);
-    if (st == JB_OK) {
-        const bool sm = K <= PF_SMEM_K;
-#define JB_PF_LAUNCH(KD, SM)                                                                                       \
-    pushforward_kernel<KD, SM><<<p.grid, EV_BLOCK, 0, c->stream>>>(p.d_cols, count, p.e_hi(), p.e_lo(), p.n_lo, p.rows, \
-                                                                    p.rpb, (uint32_t)K, p.d_lanes, p.bad())
-        if (kind == SK_U8) { if (sm) JB_PF_LAUNCH(SK_U8, true); else JB_PF_LAUNCH(SK_U8, false); }
-        else { if (sm) JB_PF_LAUNCH(SK_U16, true); else JB_PF_LAUNCH(SK_U16, false); }
-#undef JB_PF_LAUNCH
-        c->launches++;
-        st = c->check(cudaGetLastError(), "pushforward_kernel launch");
-    }
-    unsigned int flag = 0;
-    if (st == JB_OK) st = c->check(cudaMemcpyAsync(&flag, p.bad(), 4, cudaMemcpyDeviceToHost, c->stream), "pushforward flag D2H");
-    if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "pushforward sync");
-    if (st == JB_OK && flag) st = fail_bad_address(c);
-    // the tables are created only once the bins are known to be valid
-    std::vector<jb_table> made;
-    for (size_t i = 0; i < count && st == JB_OK; ++i) {
-        Table t;
-        st = c->dev_alloc((void**)&t.buf, K * 32);
-        if (st != JB_OK) break;
-        t.cap = t.len = K;
-        const jb_table h = c->next_id++;
-        c->tables[h] = t;
-        made.push_back(h);
-        bins_to_fr_kernel<<<launch_grid(c, K, BINS_BLOCK, 8), BINS_BLOCK, 0, c->stream>>>(p.d_lanes + i * K * 8, K, t.buf);
-        c->launches++;
-        st = c->check(cudaGetLastError(), "bins_to_fr_kernel launch");
-    }
+    if (st == JB_OK) st = one_hot_pushforward_into(c, dcols.data(), count, kind, T, K, r_cycle, bufs.data());
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "pushforward tables sync");
     if (st != JB_OK) {
-        for (jb_table h : made) {
-            c->release(c->tables[h]);
-            c->tables.erase(h);
-        }
+        for (Table& t : made) c->release(t);
         return st;
     }
-    std::memcpy(out_tables, made.data(), count * sizeof(jb_table));
+    for (size_t i = 0; i < count; ++i) {
+        out_tables[i] = c->next_id++;
+        c->tables[out_tables[i]] = made[i];
+    }
     return JB_OK;
 }
 
