@@ -81,10 +81,25 @@ typedef uint64_t jb_srs;            /* device-resident affine G1 bases (HyperKZG
 const char* jb_version(void);
 const char* jb_status_str(int status);
 int jb_device_count(void);
+/* Stream ordering of device memory the caller hands in or reads back (borrowed tables, device columns and scalars,
+ * tables bound in place, exported tables, new tables read through jb_table_device_ptr):
+ *  - Every device read and write of a call is enqueued on the context's stream; calls that return host values wait
+ *    for their own work, calls that return device data do not.
+ *  - Device memory passed in must be complete when the context's stream reaches the call. Nothing is ordered against
+ *    other streams for the caller: a jb_ctx_create context owns a cudaStreamNonBlocking stream, which waits neither
+ *    for the legacy default stream nor for any other stream. Make it wait (cudaEventRecord on the producing stream,
+ *    cudaStreamWaitEvent on jb_ctx_stream) or create the context on the producing stream.
+ *  - Device results are complete in the order of the context's stream: a consumer on another stream must wait for
+ *    it the same way before it reads them.
+ *  - Borrowed device memory must stay allocated, and must not be reused by the caller's allocator, until the context's
+ *    stream has finished the work that reads or writes it (a caching allocator that tracks only its own streams, such as
+ *    torch's, needs the same event, or a reference kept until then). */
 /* ProofSession::new - owns a stream and memory pools on `device`. */
 int jb_ctx_create(int device, jb_ctx** out);
 /* Same, but enqueues on a caller-owned cudaStream_t (e.g. torch's current stream). */
 int jb_ctx_create_on_stream(int device, void* cuda_stream, jb_ctx** out);
+/* The cudaStream_t the context enqueues on (its own, or the caller's; NULL = the legacy default stream). */
+int jb_ctx_stream(jb_ctx* ctx, void** out);
 void jb_ctx_destroy(jb_ctx* ctx);
 const char* jb_last_error(jb_ctx* ctx);
 int jb_ctx_synchronize(jb_ctx* ctx);

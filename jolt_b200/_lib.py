@@ -22,6 +22,7 @@ SIGNATURES = {
     "jb_device_count": (ctypes.c_int, []),
     "jb_ctx_create": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(c_void_p)]),
     "jb_ctx_create_on_stream": (ctypes.c_int, [ctypes.c_int, c_void_p, ctypes.POINTER(c_void_p)]),
+    "jb_ctx_stream": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "jb_ctx_destroy": (None, [c_void_p]),
     "jb_last_error": (ctypes.c_char_p, [c_void_p]),
     "jb_ctx_synchronize": (ctypes.c_int, [c_void_p]),

@@ -6,6 +6,7 @@ All table-sized data stays on the device; only O(rounds * degree) values cross b
 from __future__ import annotations
 
 import ctypes
+import sys
 from dataclasses import dataclass, field as dc_field
 
 import numpy as np
@@ -37,7 +38,18 @@ class SumcheckError(RuntimeError):
 
 
 class Session:
-    """Device half of ProofSession (crates/jolt-kernels/src/backend.rs:283-286)."""
+    """Device half of ProofSession (crates/jolt-kernels/src/backend.rs:283-286).
+
+    Work is enqueued on the session's stream: its own non-blocking stream (cuda_stream=None), or the caller's
+    (e.g. torch.cuda.current_stream().cuda_stream; 0 is the legacy default stream). When that is not torch's current
+    stream, the two are ordered here: CUDA tensors handed in (wrap_device, device columns) are read after the work
+    torch's current stream has enqueued so far, and device data handed back (tables bound in place, new tables, exported
+    tables, device_ptr) is written before the work torch's current stream enqueues next. A borrowed table written on
+    another stream after wrap_device must be ordered by the caller (after_torch, or its own events). A borrowed tensor
+    (wrap_device, device columns, export_table's destination) must stay alive until the session's stream is done with
+    it: torch's caching allocator only follows torch's streams, so a tensor freed earlier may be handed out and written
+    again while the session still reads or writes it. Keep a reference until a before_torch() on the tensor's stream
+    or a synchronize()."""
 
     def __init__(self, device: int = 0, cuda_stream: int | None = None):
         self.lib = _lib.load()
@@ -50,6 +62,36 @@ class Session:
             raise JoltB200Error(st, self.lib.jb_status_str(st).decode())
         self.h = h
         self.device = device
+        p = ctypes.c_void_p()
+        self.check(self.lib.jb_ctx_stream(h, ctypes.byref(p)))
+        self.stream = p.value or 0  # the cudaStream_t the session enqueues on
+
+    def _torch_streams(self):
+        """(the session's stream, torch's current stream) as torch streams on the session's device, or None when they
+        are one stream or torch holds no CUDA state (then nothing of torch's can be pending)."""
+        torch = sys.modules.get("torch")
+        if torch is None or not torch.cuda.is_initialized():
+            return None
+        cur = torch.cuda.current_stream(self.device)
+        if cur.cuda_stream == self.stream:
+            return None
+        own = (torch.cuda.default_stream(self.device) if self.stream == 0
+               else torch.cuda.ExternalStream(self.stream, device=self.device))
+        return own, cur
+
+    def after_torch(self):
+        """Makes the session's next work wait for the work enqueued on torch's current stream so far (one event, no
+        host synchronisation)."""
+        s = self._torch_streams()
+        if s is not None:
+            s[0].wait_stream(s[1])
+
+    def before_torch(self):
+        """Makes the work torch's current stream enqueues next wait for the session's work so far (one event, no host
+        synchronisation)."""
+        s = self._torch_streams()
+        if s is not None:
+            s[1].wait_stream(s[0])
 
     def check(self, st: int):
         if st != _lib.JB_OK:
@@ -197,6 +239,9 @@ class Polynomial:
 
     @classmethod
     def wrap_device(cls, session: Session, device_ptr: int, length: int) -> "Polynomial":
+        """Borrows `length` field entries of caller-owned device memory (e.g. a torch tensor's data_ptr()), read after
+        the work torch's current stream has enqueued so far."""
+        session.after_torch()
         h = ctypes.c_uint64()
         session.check(session.lib.jb_table_wrap_device(session.h, ctypes.c_void_p(device_ptr), length, ctypes.byref(h)))
         return cls(session, h.value)
@@ -212,11 +257,13 @@ class Polynomial:
     def device_ptr(self) -> int:
         p = ctypes.c_void_p()
         self.s.check(self.s.lib.jb_table_device_ptr(self.s.h, self.handle, ctypes.byref(p)))
+        self.s.before_torch()
         return p.value
 
     def bind_with_order(self, scalar, order: int = HIGH_TO_LOW) -> None:
         r = _limbs(scalar)
         self.s.check(self.s.lib.jb_table_bind(self.s.h, self.handle, _p(r), order))
+        self.s.before_torch()  # a borrowed table is bound in place
 
     def bind(self, scalar, order: int = HIGH_TO_LOW) -> None:
         """Polynomial::bind == HighToLow (dense.rs:169-171); the legacy signature passes the order."""
@@ -257,9 +304,12 @@ class Polynomial:
             raise ValueError("linear_combination: at least one term")
         n = max(t.length for t in terms) if length is None else length
         arr, keep = LinearTerm._array(terms)
+        if any(t.on_device for t in terms):
+            session.after_torch()
         h = ctypes.c_uint64()
         session.check(session.lib.jb_table_linear_combination(session.h, ctypes.cast(arr, ctypes.c_void_p), len(terms),
                                                               n, ctypes.byref(h)))
+        session.before_torch()
         return Polynomial(session, h.value)
 
     @staticmethod
@@ -273,9 +323,12 @@ class Polynomial:
             raise ValueError("vector_matrix_product: at least one term")
         n = max(t.length for t in terms) if length is None else length
         arr, keep = LinearTerm._array(terms)
+        if any(t.on_device for t in terms):
+            session.after_torch()
         h = ctypes.c_uint64()
         session.check(session.lib.jb_lc_vector_matrix_product(session.h, ctypes.cast(arr, ctypes.c_void_p), len(terms),
                                                               n, row_width, left.handle, ctypes.byref(h)))
+        session.before_torch()
         return Polynomial(session, h.value)
 
     @staticmethod
@@ -357,6 +410,8 @@ def evaluate_small(session: Session, columns, point, kinds=None) -> list[int]:
         raise ValueError("evaluate_small: columns must have one length")
     pt = point_limbs(point)
     out = np.empty((len(columns), 4), dtype=np.uint64)
+    if on_device[0]:
+        session.after_torch()
     session.check(session.lib.jb_small_evaluate_batch(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs),
                                                       (ctypes.c_int * len(ks))(*ks), lens[0], on_device[0],
                                                       _p(pt), pt.shape[0], _p(out)))
@@ -402,6 +457,8 @@ def one_hot_evaluate(session: Session, columns, K: int, point, layout: str = "cy
     if K < 1 or T < 1 or pt.shape[0] != (K * T).bit_length() - 1:
         raise ValueError("one_hot_evaluate: the point must have log2(K T) coordinates")
     out = np.empty((len(ptrs), 4), dtype=np.uint64)
+    if dev:
+        session.after_torch()
     session.check(session.lib.jb_one_hot_evaluate(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs), kind, T, K,
                                                   ONE_HOT_LAYOUTS[layout], dev, _p(pt), _p(out)))
     return F.limbs_to_ints(out)
@@ -418,8 +475,11 @@ def one_hot_pushforward(session: Session, columns, K: int, r_cycle) -> list[Poly
     if pt.shape[0] != T.bit_length() - 1:
         raise ValueError("one_hot_pushforward: r_cycle must have log2(T) coordinates")
     out = np.zeros(len(ptrs), dtype=np.uint64)
+    if dev:
+        session.after_torch()
     session.check(session.lib.jb_one_hot_pushforward(session.h, (ctypes.c_void_p * len(ptrs))(*ptrs), len(ptrs), kind,
                                                      T, K, dev, _p(pt), _p(out)))
+    session.before_torch()
     return [Polynomial(session, int(h)) for h in out]
 
 
@@ -433,6 +493,7 @@ class EqPolynomial:
         h = ctypes.c_uint64()
         session.check(session.lib.jb_eq_evals(session.h, _p(r) if r.shape[0] else None, r.shape[0],
                                                _p(sc) if sc is not None else None, ctypes.byref(h)))
+        session.before_torch()
         return Polynomial(session, h.value)
 
     @staticmethod
@@ -441,6 +502,7 @@ class EqPolynomial:
         h = ctypes.c_uint64()
         session.check(session.lib.jb_eq_evals_aligned_block(session.h, _p(r), r.shape[0], start_index, block_size,
                                                              ctypes.byref(h)))
+        session.before_torch()
         return Polynomial(session, h.value)
 
 
@@ -450,6 +512,7 @@ def _structured_evals(session: Session, fn, r_limbs, scaling_factor) -> Polynomi
     h = ctypes.c_uint64()
     session.check(fn(session.h, _p(r) if r.shape[0] else None, r.shape[0], _p(sc) if sc is not None else None,
                      ctypes.byref(h)))
+    session.before_torch()
     return Polynomial(session, h.value)
 
 
@@ -613,6 +676,19 @@ class ProductMember:
         out = np.empty((self.m, 4), dtype=np.uint64)
         self.s.check(self.s.lib.jb_member_final_evals(self.h, _p(out)))
         return out if raw else F.limbs_to_ints(out)
+
+    def export_table(self, j: int, dst) -> int:
+        """Copies table j's current (possibly partly bound) entries into `dst`, a contiguous CUDA tensor of at least
+        that many 32-byte entries (jb_member_export_table); returns the number of entries. The copy is ordered after
+        torch's current stream's work so far and before its next."""
+        if not (_is_device_tensor(dst) and dst.is_contiguous()):
+            raise ValueError("export_table: the destination must be a contiguous CUDA tensor")
+        n = ctypes.c_size_t()
+        self.s.after_torch()
+        self.s.check(self.s.lib.jb_member_export_table(self.h, j, ctypes.c_void_p(dst.data_ptr()),
+                                                       dst.numel() * dst.element_size() // 32, ctypes.byref(n)))
+        self.s.before_torch()
+        return n.value
 
     def close(self):
         if self.h:
@@ -807,6 +883,8 @@ class ExpressionMember(ProductMember):
         mons = _monomials_c(monomials)
         w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
         sc = None if scale is None else _limbs(scale)
+        if any(s.on_device for s in sources):
+            session.after_torch()
         h = ctypes.c_void_p()
         session.check(session.lib.jb_member_create_expr_sources(
             session.h, ctypes.cast(arr, ctypes.c_void_p), len(sources), lens.pop(), ctypes.cast(mons, ctypes.c_void_p),
@@ -848,6 +926,8 @@ class ProductSourcesMember(ExpressionMember):
             src._fill(arr[i], keep)
         w = None if w_limbs is None else np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
         sc = None if scale is None else _limbs(scale)
+        if any(s.on_device for s in sources):
+            session.after_torch()
         h = ctypes.c_void_p()
         session.check(session.lib.jb_member_create_product_sources(
             session.h, ctypes.cast(arr, ctypes.c_void_p), len(sources), lens.pop() if lens else 0,
@@ -894,6 +974,8 @@ class ReadWriteCheckingMember(ExpressionMember):
         src(init)._fill(init_c, keep)
         w = point_limbs(w_cycle)
         sc = None if scale is None else _limbs(scale)
+        if dev or any(isinstance(k, Source) and k.on_device for k in keep):
+            session.after_torch()
         h = ctypes.c_void_p()
         session.check(session.lib.jb_member_create_read_write(
             session.h, ctypes.cast(arr, ctypes.c_void_p), len(accesses), write, kind, dev, T, K,
@@ -927,6 +1009,8 @@ class BooleanityMember(ExpressionMember):
             cf[i] = _limbs(c % F.R_MOD if isinstance(c, (int, np.integer)) else c)
         ra, rc = point_limbs(r_addr), point_limbs(r_cycle)
         sc = None if scale is None else _limbs(scale)
+        if dev:
+            session.after_torch()
         h = ctypes.c_void_p()
         session.check(session.lib.jb_member_create_booleanity(
             session.h, (ctypes.c_void_p * max(len(ptrs), 1))(*ptrs), len(ptrs), kind, dev, T, K, _p(cf),

@@ -234,6 +234,12 @@ void jb_ctx_destroy(jb_ctx* c) {
     delete c;
 }
 
+int jb_ctx_stream(jb_ctx* c, void** out) {
+    if (!c || !out) return JB_ERR_INVALID;
+    *out = (void*)c->stream;
+    return JB_OK;
+}
+
 const char* jb_last_error(jb_ctx* c) { return c ? c->err.c_str() : "null context"; }
 
 int jb_ctx_synchronize(jb_ctx* c) {
