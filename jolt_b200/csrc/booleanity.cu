@@ -281,19 +281,14 @@ int bool_create(jb_ctx* c, const void* const* columns, size_t count, int kind, i
     if (scale && !canonical_fr(scale)) return c->fail(JB_ERR_INVALID, "booleanity: scale not canonical");
 
     // everything the rounds need is allocated here
-    jb_member* mem = new (std::nothrow) jb_member();
+    jb_member* mem = new_member(c, MemberKind::Booleanity, 2, 1, order, K * T);
     if (!mem) return JB_ERR_OOM;
     BoolState* bl = new (std::nothrow) BoolState();
     if (!bl) {
         delete mem;
         return JB_ERR_OOM;
     }
-    mem->ctx = c;
     mem->bl = bl;
-    mem->m = 2;
-    mem->order = order;
-    mem->rounds = log_k + log_t;
-    mem->len = K * T;
     bl->d = (int)count;
     bl->kind = kind;
     bl->order = order;

@@ -142,6 +142,19 @@ int dispatch_expr(jb_ctx* c, const jb_member* mem, bool weighted, bool skip1, co
 
 }  // namespace
 
+jb_member* new_member(jb_ctx* c, MemberKind kind, int m, int terms, int order, size_t len) {
+    jb_member* mem = new (std::nothrow) jb_member();
+    if (!mem) return nullptr;
+    mem->ctx = c;
+    mem->kind = kind;
+    mem->m = m;
+    mem->terms = terms;
+    mem->order = order;
+    mem->len = len;
+    mem->rounds = (size_t)log2_of(len);
+    return mem;
+}
+
 extern "C" {
 
 // ---- sumcheck member -------------------------------------------------------------------
@@ -162,17 +175,10 @@ static int check_tables(jb_ctx* c, const jb_table* handles, size_t T, size_t* le
 }
 
 // A new member owning the T checked tables (context lock held).
-static int adopt_tables(jb_ctx* c, const jb_table* handles, size_t T, size_t len, int m, int terms, int order,
-                        jb_member** out) {
-    jb_member* mem = new (std::nothrow) jb_member();
+static int adopt_tables(jb_ctx* c, MemberKind kind, const jb_table* handles, size_t T, size_t len, int m, int terms,
+                        int order, jb_member** out) {
+    jb_member* mem = new_member(c, kind, m, terms, order, len);
     if (!mem) return JB_ERR_OOM;
-    mem->ctx = c;
-    mem->m = m;
-    mem->terms = terms;
-    mem->order = order;
-    mem->len = len;
-    mem->rounds = 0;
-    while (((size_t)1 << mem->rounds) < len) ++mem->rounds;
     for (size_t j = 0; j < T; ++j) {
         auto it = c->tables.find(handles[j]);
         mem->tables.push_back(it->second);
@@ -192,7 +198,7 @@ static int member_create_common(jb_ctx* c, const jb_table* handles, size_t m, si
     size_t len = 0;
     int st = check_tables(c, handles, T, &len);
     if (st != JB_OK) return st;
-    return adopt_tables(c, handles, T, len, (int)m, (int)terms, order, out);
+    return adopt_tables(c, MemberKind::Dense, handles, T, len, (int)m, (int)terms, order, out);
 }
 
 int jb_member_create(jb_ctx* c, const jb_table* handles, size_t m, int order, jb_member** out) {
@@ -209,9 +215,15 @@ int jb_member_num_rounds(jb_member* mem, size_t* rounds) {
     return JB_OK;
 }
 
+// Whether the member's rounds take the split-eq host step (eq_prove_round): a member with split-eq weighting, and every
+// read-write and booleanity member (a booleanity member with T = 1 has no eq tables, only its address rounds' factor).
+static bool eq_rounds(const jb_member* mem) {
+    return mem->eq || mem->kind == MemberKind::ReadWrite || mem->kind == MemberKind::Booleanity;
+}
+
 int jb_member_degree(jb_member* mem, size_t* degree) {
     if (!mem || !degree) return JB_ERR_INVALID;
-    *degree = (size_t)mem->m + (mem->eq ? 1 : 0);
+    *degree = (size_t)mem->m + (eq_rounds(mem) ? 1 : 0);
     return JB_OK;
 }
 
@@ -219,7 +231,7 @@ jb_ctx* jb_member_context(jb_member* mem) { return mem ? mem->ctx : nullptr; }
 
 int jb_member_num_tables(jb_member* mem, size_t* tables) {
     if (!mem || !tables) return JB_ERR_INVALID;
-    *tables = mem->bl ? (size_t)mem->bl->d : (size_t)mem->ntables();
+    *tables = (size_t)mem->ntables();
     return JB_OK;
 }
 
@@ -300,25 +312,25 @@ static int member_round(jb_member* mem, const uint64_t* bind, bool skip1, void* 
             outs[j] = t.alt;
         }
     }
-    if (!mem->product)
+    if (mem->kind != MemberKind::Product)
         for (int j = 0; j < T; ++j) {
             tp.in[j] = ins[j];
             tp.out[j] = outs[j];
         }
-    const RoundOut ro = round_out(c, lanes_out, slot, seq_out);
-    int st;
-    if (mem->product) {
-        st = product_round(c, mem, ins, outs, eqr, eqr ? true : skip1, pairs, do_bind, hi4, s, ro);
-    } else if (eqr) {
+    if (eqr) {
         tp.e_out = eqr->e_out;
         tp.e_in = eqr->e_in;
         tp.in_bits = eqr->in_bits;
-        st = mem->expr ? dispatch_expr(c, mem, true, true, tp, pairs, do_bind, hi4, s, ro)
-                       : dispatch_weighted(c, mem->m, mem->order, tp, pairs, do_bind, hi4, s, ro);
-    } else {
-        st = mem->expr ? dispatch_expr(c, mem, false, skip1, tp, pairs, do_bind, hi4, s, ro)
-                       : dispatch_fused(c, mem->m, mem->terms, mem->order, skip1, tp, pairs, do_bind, hi4, s, ro);
     }
+    const RoundOut ro = round_out(c, lanes_out, slot, seq_out);
+    int st;
+    if (mem->kind == MemberKind::Product)
+        st = product_round(c, mem, ins, outs, eqr, eqr ? true : skip1, pairs, do_bind, hi4, s, ro);
+    else if (mem->kind == MemberKind::Dense)
+        st = eqr ? dispatch_weighted(c, mem->m, mem->order, tp, pairs, do_bind, hi4, s, ro)
+                 : dispatch_fused(c, mem->m, mem->terms, mem->order, skip1, tp, pairs, do_bind, hi4, s, ro);
+    else  // Expr, and a ReadWrite member's address rounds (a Booleanity member has passes of its own)
+        st = dispatch_expr(c, mem, eqr != nullptr, eqr ? true : skip1, tp, pairs, do_bind, hi4, s, ro);
     if (st != JB_OK) return st;
     if (do_bind) {
         for (int j = 0; j < T; ++j) {
@@ -432,6 +444,18 @@ static const uint64_t* slot_values(const uint64_t* slot, int M, bool skip1, uint
     std::memcpy(buf, slot, 64 * 8);
     std::memcpy(buf + 64, slot + 72, (size_t)(k - 16) * 32);
     return buf;
+}
+
+// One round through a launched pass: binds `bind` (if given), sweeps into result slot 0, waits for it and assembles
+// s(0..m). The caller counts the round.
+static int launched_round(jb_member* mem, const uint64_t* bind, bool skip1, const uint64_t* claim, size_t round,
+                          uint64_t* out_evals) {
+    jb_ctx* c = mem->ctx;
+    int st = member_round(mem, bind, skip1, nullptr);
+    if (st == JB_OK) st = wait_round_result0(c);
+    if (st != JB_OK) return st;
+    uint64_t vals[JB_MAX_ROUND_EVALS * 4];
+    return assemble_evals(c, mem->m, skip1, slot_values(c->h_result, mem->m, skip1, vals), claim, round, out_evals);
 }
 
 int jb_round_evals_from_kernel_values(int m, int skip_t1, const uint64_t* kernel_values, const uint64_t* claim_or_null,
@@ -567,12 +591,9 @@ static int run_round(jb_ctx* c, ResidentRun* run, RunItem* items, int n, const u
         st = resident_recover(run);
         if (st != JB_OK) return st;
         for (int i = 0; i < n; ++i) {
-            jb_member* m = items[i].mem;
-            st = member_round(m, nullptr, true, nullptr);
-            if (st == JB_OK) st = wait_round_result0(c);
-            if (st == JB_OK) st = assemble_evals(c, m->m, true, c->h_result, items[i].claim, items[i].round, items[i].out_evals);
+            st = launched_round(items[i].mem, nullptr, true, items[i].claim, items[i].round, items[i].out_evals);
             if (st != JB_OK) return st;
-            m->rounds_done++;
+            items[i].mem->rounds_done++;
         }
         return JB_OK;
     }
@@ -626,6 +647,16 @@ static void before_launch(jb_member* mem) {
     mem->ctx->quiesce_resident(false);
 }
 
+// The checks of a round's arguments that every entry point makes first, in this order (context lock held).
+static int check_round_args(jb_member* mem, const uint64_t* bind, size_t round) {
+    jb_ctx* c = mem->ctx;
+    if (round != mem->rounds_done) return c->fail(JB_ERR_INVALID, "prove_round: round index out of sequence");
+    if ((mem->rounds_done == 0) != (bind == nullptr))
+        return c->fail(JB_ERR_INVALID, "prove_round: bind must be absent exactly on the first round");
+    if (bind && !canonical_fr(bind)) return c->fail(JB_ERR_INVALID, "prove_round: challenge limbs not canonical");
+    return JB_OK;
+}
+
 int jb_member_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim,
                           uint64_t* out_evals) {
     if (!mem || !out_evals) return JB_ERR_INVALID;
@@ -636,16 +667,14 @@ int jb_member_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
         return st;
     }
     Guard g(c, true);
-    if (round != mem->rounds_done) return c->fail(JB_ERR_INVALID, "prove_round: round index out of sequence");
-    if ((mem->rounds_done == 0) != (bind == nullptr))
-        return c->fail(JB_ERR_INVALID, "prove_round: bind must be absent exactly on the first round");
-    if (bind && !canonical_fr(bind)) return c->fail(JB_ERR_INVALID, "prove_round: challenge limbs not canonical");
+    int st = check_round_args(mem, bind, round);
+    if (st != JB_OK) return st;
     if (mem->len < (bind ? 4u : 2u))
         return c->fail(JB_ERR_INVALID, bind ? "prove_round: no round left after this bind (use finish_rounds)"
                                             : "prove_round: member is fully bound");
-    if (mem->eq) {
+    if (eq_rounds(mem)) {
         before_launch(mem);
-        int st = eq_prove_round(mem, bind, round, claim, out_evals);
+        st = eq_prove_round(mem, bind, round, claim, out_evals);
         if (st == JB_OK) mem->rounds_done++;
         return st;
     }
@@ -653,19 +682,13 @@ int jb_member_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     // kernel skips t = 1 and s(1) = claim - s(0); with verification on (or no claim) it computes
     // every point and the claim, if given, is checked (the reference tier, naive.rs:301-308).
     const bool skip1 = claim != nullptr && !c->verify_rounds;
-    int st;
     if (skip1) {
         // the resident kernel serves this and every later round of the member: no launch per round
         st = resident_member_prove(mem, bind, claim, round, false, out_evals);  // (counts the round itself)
         if (st != JB_ERR_UNSUPPORTED) return st;
     }
     before_launch(mem);
-    st = member_round(mem, bind, skip1, nullptr);
-    if (st != JB_OK) return st;
-    st = wait_round_result0(c);
-    if (st != JB_OK) return st;
-    uint64_t vals[JB_MAX_ROUND_EVALS * 4];
-    st = assemble_evals(c, mem->m, skip1, slot_values(c->h_result, mem->m, skip1, vals), claim, round, out_evals);
+    st = launched_round(mem, bind, skip1, claim, round, out_evals);
     if (st == JB_OK) mem->rounds_done++;
     return st;
 }
@@ -689,8 +712,8 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     jb_ctx* c = mem->ctx;
     if (!claim) return c->fail(JB_ERR_INVALID, "eq member: the running claim is required (Gruen hint s(0)+s(1))");
     const size_t n = mem->eq_n;
-    if (mem->rw && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
-    if (mem->bl) {  // the address rounds come first; the cycle rounds are this member's eq rounds
+    if (mem->kind == MemberKind::ReadWrite && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
+    if (mem->kind == MemberKind::Booleanity) {  // the address rounds come first; the cycle rounds are its eq rounds
         const size_t ka = mem->bl->log_k;
         if (round < ka) return bool_address_round(mem, bind, round, claim, out_evals);
         if (round == ka && bind) {  // the last address variable
@@ -736,9 +759,9 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     const HostFr wc = HostFr::from_limbs(mem->eq_w.data() + 4 * cur_var);
     const HostFr l1 = scalar * wc, l0 = scalar - l1;
     if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
-    int st = mem->rw   ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
-             : mem->bl ? bool_cycle_pass(mem, bind, er, round_out(c, nullptr, 0, nullptr))
-                       : member_round(mem, bind, true, nullptr, &er);
+    int st = mem->kind == MemberKind::ReadWrite    ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+             : mem->kind == MemberKind::Booleanity ? bool_cycle_pass(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+                                                   : member_round(mem, bind, true, nullptr, &er);
     if (st != JB_OK) return st;
     return eq_round_tail(mem, l0, l1, claim, round, out_evals);
 }
@@ -895,9 +918,8 @@ static int check_expr(jb_ctx* c, size_t ntables, const jb_monomial* monomials, s
     return JB_OK;
 }
 
-// Makes `mem` an expression member: the kernel parameter form of the checked monomials.
+// The kernel parameter form of the checked monomials into mem->ex.
 static void make_expr(jb_member* mem, const jb_monomial* monomials, size_t nmonomials, size_t ntables, int D) {
-    mem->expr = true;
     ExprParams& ex = mem->ex;
     std::memset(&ex, 0, sizeof ex);
     const HostFr one = HostFr::one(), minus_one = HostFr::zero() - one;
@@ -940,7 +962,7 @@ int jb_member_create_expr(jb_ctx* c, const jb_table* handles, size_t ntables, co
             return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
         own_pass = !blocks || (eq_w_or_null ? !(nmonomials == 1 && D <= 3) : !shape_supported(D, (int)nmonomials));
         if (own_pass) {
-            st = adopt_tables(c, handles, ntables, len, D, 1, order, out);
+            st = adopt_tables(c, MemberKind::Expr, handles, ntables, len, D, 1, order, out);
             if (st != JB_OK) return st;
             make_expr(*out, monomials, nmonomials, ntables, D);
         }
@@ -981,13 +1003,13 @@ static void discard_sources(jb_member* mem) {
 }
 
 // The creation of a member over sources (expression or product): under the context lock, `check` (the relation's own
-// checks, which return its status first), then the sources, then everything the rounds need is allocated and
-// `shape` makes the new member the relation's member; check sets the member's degree without eq.
+// checks, which return its status first), then the sources, then everything the rounds need is allocated; check sets
+// the member's degree without eq.
 }  // extern "C"
-template <class Check, class Shape>
-static int create_over_sources(jb_ctx* c, const jb_source* sources, size_t nsources, size_t len,
+template <class Check>
+static int create_over_sources(jb_ctx* c, MemberKind kind, const jb_source* sources, size_t nsources, size_t len,
                                const uint64_t* eq_w_or_null, size_t nvars, const uint64_t* eq_scale_or_null, int order,
-                               Check check, Shape shape, jb_member** out) {
+                               Check check, jb_member** out) {
     jb_member* mem = nullptr;
     int st = JB_OK;
     {
@@ -1006,14 +1028,8 @@ static int create_over_sources(jb_ctx* c, const jb_source* sources, size_t nsour
                     return c->fail(JB_ERR_INVALID, "member: duplicate table handle");
         }
         // everything is allocated here: the columns, the eq tables, the len/2 outputs, the LowToHigh ping-pong buffers
-        mem = new (std::nothrow) jb_member();
+        mem = new_member(c, kind, D, 1, order, len);
         if (!mem) return JB_ERR_OOM;
-        mem->ctx = c;
-        mem->m = D;
-        mem->order = order;
-        mem->len = len;
-        mem->rounds = (size_t)log2_of(len);
-        shape(mem);
         mem->tables.resize(nsources);
         mem->src.resize(nsources);
         unsigned int* d_flag = nullptr;
@@ -1076,8 +1092,10 @@ int jb_member_create_expr_sources(jb_ctx* c, const jb_source* sources, size_t ns
         *D_out = D;
         return st;
     };
-    auto shape = [&](jb_member* mem) { make_expr(mem, monomials, nmonomials, nsources, D); };
-    return create_over_sources(c, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null, order, check, shape, out);
+    const int st = create_over_sources(c, MemberKind::Expr, sources, nsources, len, eq_w_or_null, nvars,
+                                       eq_scale_or_null, order, check, out);
+    if (st == JB_OK) make_expr(*out, monomials, nmonomials, nsources, D);
+    return st;
 }
 
 // ---- product member over sources ------------------------------------------------------------------------
@@ -1102,16 +1120,16 @@ int jb_member_create_product_sources(jb_ctx* c, const jb_source* sources, size_t
         *D_out = (int)nsources;
         return (int)JB_OK;
     };
-    auto shape = [&](jb_member* mem) { mem->product = true; };
-    return create_over_sources(c, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null, order, check, shape, out);
+    return create_over_sources(c, MemberKind::Product, sources, nsources, len, eq_w_or_null, nvars, eq_scale_or_null,
+                               order, check, out);
 }
 
 // ---- read-write checking member -------------------------------------------------------------------------
-// Binds a cycle variable of a read-write member (its eq factor has absorbed r); after the last one the member becomes
-// an expression member over its K-entry tables ra_0 .. ra_{A-1}, Val, inc: sum_k e sum_a c_a ra_a(k) (Val(k) + d_a inc)
-// with e = scale * eq(w_cycle, r_cycle), as monomials c_a e ra_a Val and c_a e ra_a inc.
+// Binds a cycle variable of a read-write member (its eq factor has absorbed r); after the last one the member's address
+// rounds are the expression pass over its K-entry tables ra_0 .. ra_{A-1}, Val, inc: sum_k e sum_a c_a ra_a(k) (Val(k) +
+// d_a inc) with e = scale * eq(w_cycle, r_cycle), as monomials c_a e ra_a Val and c_a e ra_a inc.
 static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
-    const RwState& rw = *mem->rw;
+    RwState& rw = *mem->rw;
     const int A = rw.A;
     int st = rw_cycle_bind(mem, r);
     if (st != JB_OK || rw.rows > 1) return st;
@@ -1128,6 +1146,7 @@ static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
             ++nm;
         }
     make_expr(mem, mo, nm, (size_t)A + 2, 2);
+    rw.cycles = false;
     return JB_OK;
 }
 
@@ -1141,12 +1160,7 @@ static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, 
         if (st != JB_OK) return st;
         bind = nullptr;
     }
-    const bool skip1 = !c->verify_rounds;
-    int st = member_round(mem, bind, skip1, nullptr);
-    if (st == JB_OK) st = wait_round_result0(c);
-    if (st != JB_OK) return st;
-    uint64_t vals[JB_MAX_ROUND_EVALS * 4];
-    st = assemble_evals(c, 2, skip1, slot_values(c->h_result, 2, skip1, vals), claim, round, out_evals);  // s(0..2)
+    const int st = launched_round(mem, bind, !c->verify_rounds, claim, round, out_evals);  // s(0..2)
     if (st != JB_OK) return st;
     const RoundConsts& rc = round_consts(2);
     HostFr s3 = HostFr::zero();
@@ -1199,14 +1213,14 @@ int jb_member_create_booleanity(jb_ctx* c, const void* const* columns, size_t co
     }
     *out = mem;
     if (T >= 2) return eq_setup(mem, r_cycle, mem->bl->log_t, scale_or_null, out);
-    mem->eq = true;  // T = 1: address rounds only, no cycle eq tables
+    // T = 1: address rounds only, no cycle eq tables
     (scale_or_null ? HostFr::from_limbs(scale_or_null) : HostFr::one()).store(mem->eq_scalar);
     return JB_OK;
 }
 
 // eq(w, r) * scale after all rounds (the member's eq factor of the final claim)
 int jb_eq_member_scalar(jb_member* mem, uint64_t out[4]) {
-    if (!mem || !out || !mem->eq) return JB_ERR_INVALID;
+    if (!mem || !out || !eq_rounds(mem)) return JB_ERR_INVALID;
     std::memcpy(out, mem->eq_scalar, 32);
     return JB_OK;
 }
@@ -1223,15 +1237,8 @@ static __global__ void __launch_bounds__(256) interleave_shards_kernel(const uin
 static int gather_into_tail(jb_member* mem) {  // called with the context lock held
     jb_ctx* c = mem->ctx;
     const size_t len = mem->len, G = (size_t)c->world;
-    jb_member* tail = new (std::nothrow) jb_member();
+    jb_member* tail = new_member(c, MemberKind::Dense, mem->m, mem->terms, mem->order, len * G);
     if (!tail) return JB_ERR_OOM;
-    tail->ctx = c;
-    tail->m = mem->m;
-    tail->terms = mem->terms;
-    tail->order = mem->order;
-    tail->len = len * G;
-    tail->rounds = 0;
-    while (((size_t)1 << tail->rounds) < tail->len) ++tail->rounds;
     int st = JB_OK;
     for (int j = 0; j < mem->ntables() && st == JB_OK; ++j) {
         Table t;
@@ -1281,10 +1288,7 @@ static int sharded_prove_round(jb_member* mem, const uint64_t* bind, size_t roun
                 if (st != JB_ERR_UNSUPPORTED) return st;
             }
             before_launch(mem);
-            st = member_round(mem, bind, skip1, nullptr);
-            if (st == JB_OK) st = wait_round_result0(c);
-            if (st != JB_OK) return st;
-            return assemble_evals(c, mem->m, skip1, c->h_result, claim, round, out_evals);
+            return launched_round(mem, bind, skip1, claim, round, out_evals);
         }
         if (!mem->tail) {
             const size_t len_after = bind ? mem->len / 2 : mem->len;
@@ -1371,10 +1375,10 @@ int jb_member_prove_round_partials(jb_member* mem, const uint64_t* bind, size_t 
     (void)round;
     if (!mem || !lanes_out) return JB_ERR_INVALID;
     Guard g(mem->ctx, true);
-    if (mem->expr) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: expression members are not sharded");
-    if (mem->product) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: product members are not sharded");
-    if (mem->rw) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: read-write members are not sharded");
-    if (mem->bl) return mem->ctx->fail(JB_ERR_UNSUPPORTED, "prove_round_partials: booleanity members are not sharded");
+    static const char* const names[] = {"dense", "expression", "product", "read-write", "booleanity"};  // by MemberKind
+    if (mem->kind != MemberKind::Dense)
+        return mem->ctx->fail(JB_ERR_UNSUPPORTED, (std::string("prove_round_partials: ") + names[(int)mem->kind] +
+                                                   " members are not sharded").c_str());
     before_launch(mem);
     return member_round(mem, bind, skip_t1 != 0, lanes_out);
 }
@@ -1483,9 +1487,11 @@ int jb_member_export_table(jb_member* mem, size_t j, void* device_dst, size_t ca
     jb_ctx* c = mem->ctx;
     Guard g(c, true);
     before_launch(mem);  // the host's view of the tables (buffer parity, length) is exact at a round boundary
-    if (mem->bl) return c->fail(JB_ERR_INVALID, "export_table: a booleanity member keeps its tables to itself");
+    if (mem->kind == MemberKind::Booleanity)
+        return c->fail(JB_ERR_INVALID, "export_table: a booleanity member keeps its tables to itself");
     if (j >= (size_t)mem->ntables()) return c->fail(JB_ERR_INVALID, "export_table: table index out of range");
-    if (mem->rw && !mem->expr) return c->fail(JB_ERR_INVALID, "export_table: a read-write member in its cycle rounds has no tables");
+    if (mem->kind == MemberKind::ReadWrite && mem->rw->cycles)
+        return c->fail(JB_ERR_INVALID, "export_table: a read-write member in its cycle rounds has no tables");
     if (!mem->src.empty() && mem->src[j].type != JB_SOURCE_TABLE)
         return c->fail(JB_ERR_INVALID, "export_table: the source is not bound yet (a column, not a field table)");
     if (cap_elems < mem->len) return c->fail(JB_ERR_INVALID, "export_table: destination too small");
@@ -1504,12 +1510,12 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     Guard g(c, true);
     if (mem->len < 2) return c->fail(JB_ERR_INVALID, "finish_rounds: member already fully bound");
     if (!canonical_fr(bind)) return c->fail(JB_ERR_INVALID, "finish_rounds: challenge limbs not canonical");
-    if (mem->rw && !mem->expr) {  // K = 1: the last cycle variable is the member's last
+    if (mem->kind == MemberKind::ReadWrite && mem->rw->cycles) {  // K = 1: the last cycle variable is the member's last
         if (mem->len != 2) return c->fail(JB_ERR_INVALID, "finish_rounds: rounds remain");
         eq_absorb_bind(mem, 0, bind);
         return rw_bind_cycle(mem, bind);
     }
-    if (mem->bl) {  // the last variable: a cycle variable, or the last address variable when T = 1
+    if (mem->kind == MemberKind::Booleanity) {  // the last variable: a cycle one, or the last address one when T = 1
         if (mem->len != 2) return c->fail(JB_ERR_INVALID, "finish_rounds: rounds remain");
         const BoolState& bl = *mem->bl;
         eq_absorb_coord(mem, bl.T == 1 ? bool_addr_coord(bl, bl.log_k - 1)
@@ -1519,7 +1525,7 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
         if (st == JB_OK) mem->len = 1;
         return st;
     }
-    if (mem->eq && !mem->rw) {
+    if (mem->eq && mem->kind != MemberKind::ReadWrite) {  // (a read-write member's address rounds have no eq factor)
         size_t var = 0;
         for (size_t l = mem->len; l > 2; l >>= 1) ++var;  // unbound variables besides the one being bound
         // LowToHigh binds w[var] (the most significant unbound one is w[0]); HighToLow binds w[n - 1 - var]
@@ -1530,11 +1536,13 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     if (mem->run) {
         // the terminal bind is one more mailbox command; a fully bound member gets its values back with the
         // acknowledgement (has_final), so nothing is read from the device afterwards
-        return resident_member_final(mem, bind);
+        const int st = resident_member_final(mem, bind);
+        // (a kernel found lost before the command was posted leaves the bind to the launches below)
+        if (st != JB_OK || mem->len < 2) return st;
     }
     before_launch(mem);
     if (!mem->src.empty()) {  // len = 2: the sources are bound straight from their columns
-        int st = mem->product ? product_finish(mem, bind) : sources_finish(mem, bind);
+        int st = mem->kind == MemberKind::Product ? product_finish(mem, bind) : sources_finish(mem, bind);
         if (st != JB_OK) return st;
     } else {
         for (int j = 0; j < mem->ntables(); ++j) {
@@ -1546,11 +1554,13 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
     return JB_OK;
 }
 
-static int bool_final_evals(jb_member* mem, uint64_t* out);
+// Where table j's single entry lies once the member is fully bound.
+static const uint64_t* final_entry(const jb_member* mem, int j) {
+    return mem->kind == MemberKind::Booleanity ? bool_final_entry(mem, j) : mem->tables[j].buf;
+}
 
 int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     if (!mem || !out) return JB_ERR_INVALID;
-    if (mem->bl) return bool_final_evals(mem, out);
     jb_ctx* c = mem->ctx;
     if (mem->sharded && !mem->gathered) {
         if (!mem->tail) return c->fail(JB_ERR_INVALID, "NotFullyBound (sharded member before its tail)");
@@ -1571,7 +1581,7 @@ int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     }
     before_launch(mem);
     for (int j = 0; j < T; ++j) {
-        int st = c->check(cudaMemcpyAsync(c->h_small + 4 * j, mem->tables[j].buf, 32, cudaMemcpyDeviceToHost, c->stream),
+        int st = c->check(cudaMemcpyAsync(c->h_small + 4 * j, final_entry(mem, j), 32, cudaMemcpyDeviceToHost, c->stream),
                           "final evals D2H");
         if (st != JB_OK) return st;
     }
@@ -1581,41 +1591,19 @@ int jb_member_final_evals(jb_member* mem, uint64_t* out) {
     return JB_OK;
 }
 
-// ra_0 .. ra_{d-1} of a fully bound booleanity member
-static int bool_final_evals(jb_member* mem, uint64_t* out) {
-    jb_ctx* c = mem->ctx;
-    Guard g(c, true);
-    if (mem->len != 1) {
-        char buf[96];
-        size_t remaining = 0;
-        for (size_t l = mem->len; l > 1; l >>= 1) ++remaining;
-        std::snprintf(buf, sizeof buf, "NotFullyBound { remaining: %zu }", remaining);
-        return c->fail(JB_ERR_INVALID, buf);
-    }
-    before_launch(mem);
-    const int d = mem->bl->d;
-    for (int j = 0; j < d; ++j) {
-        int st = c->check(cudaMemcpyAsync(c->h_small + 4 * j, bool_final_entry(mem, j), 32, cudaMemcpyDeviceToHost, c->stream),
-                          "final evals D2H");
-        if (st != JB_OK) return st;
-    }
-    int st = c->check(cudaStreamSynchronize(c->stream), "final evals sync");
-    if (st != JB_OK) return st;
-    std::memcpy(out, c->h_small, (size_t)d * 32);
-    return JB_OK;
-}
-
 void jb_member_destroy(jb_member* mem) {
     if (!mem) return;
     if (mem->tail) jb_member_destroy(mem->tail);
     Guard g(mem->ctx, true);
     if (mem->run) resident_end(mem->run, false);
     if (mem->eq_tabs) mem->ctx->dev_free(mem->eq_tabs);
-    sources_release(mem);
-    rw_release(mem);
-    delete mem->rw;
-    bool_release(mem);
-    delete mem->bl;
+    switch (mem->kind) {
+        case MemberKind::Expr:
+        case MemberKind::Product: sources_release(mem); break;
+        case MemberKind::ReadWrite: rw_release(mem); delete mem->rw; break;
+        case MemberKind::Booleanity: bool_release(mem); delete mem->bl; break;
+        default: break;
+    }
     for (auto& t : mem->tables) mem->ctx->release(t);
     delete mem;
 }
@@ -1654,13 +1642,13 @@ int jb_scheduler_create(jb_ctx* c, jb_member** members, size_t n, jb_scheduler**
                 delete s;
                 return c->fail(JB_ERR_INVALID, "scheduler: duplicate member");
             }
-        if (m->m + (m->eq ? 1 : 0) + 1 > JB_MAX_EVALS) {  // out_evals holds JB_MAX_EVALS elements per work item
+        if (m->m + (eq_rounds(m) ? 1 : 0) + 1 > JB_MAX_EVALS) {  // out_evals holds JB_MAX_EVALS elements per work item
             delete s;
             return c->fail(JB_ERR_UNSUPPORTED, "scheduler: a member of degree >= 8");
         }
         s->members.push_back(m);
-        if (m->sharded || m->eq || m->expr || members[0]->expr || m->product || members[0]->product || m->m != members[0]->m ||
-            m->terms != members[0]->terms || m->order != members[0]->order)
+        if (!resident_kind(m) || m->sharded || m->m != members[0]->m || m->terms != members[0]->terms ||
+            m->order != members[0]->order)
             s->homogeneous = false;
     }
     *out = s;
@@ -1710,10 +1698,8 @@ int jb_scheduler_prove_round(jb_scheduler* s, const jb_round_work* work, size_t 
         jb_member* m = s->members[w.member];
         for (size_t k = 0; k < i; ++k)
             if (work[k].member == w.member) return c->fail(JB_ERR_INVALID, "scheduler: a member appears twice in one round");
-        if (w.round != m->rounds_done) return c->fail(JB_ERR_INVALID, "prove_round: round index out of sequence");
-        if ((m->rounds_done == 0) != (w.has_bind == 0))
-            return c->fail(JB_ERR_INVALID, "prove_round: bind must be absent exactly on the first round");
-        if (w.has_bind && !canonical_fr(w.bind)) return c->fail(JB_ERR_INVALID, "prove_round: challenge limbs not canonical");
+        const int st = check_round_args(m, w.has_bind ? w.bind : nullptr, w.round);
+        if (st != JB_OK) return st;
         if (w.has_claim && !canonical_fr(w.claim)) return c->fail(JB_ERR_INVALID, "prove_round: claim limbs not canonical");
         if (m->len < (w.has_bind ? 4u : 2u)) return c->fail(JB_ERR_INVALID, "prove_round: member has no round left");
         if (!w.has_claim) all_skip1 = false;
@@ -1770,7 +1756,7 @@ static int overlapped_rounds(jb_scheduler* s, const jb_round_work* work, size_t 
         const uint64_t* bind = w.has_bind ? w.bind : nullptr;
         skip[i] = w.has_claim && !c->verify_rounds;
         via[i] = VIA_LAUNCH;
-        if (m->eq) {  // the Gruen member needs host work between its launch and its result: run it in place
+        if (eq_rounds(m)) {  // the Gruen member needs host work between its launch and its result: run it in place
             int st = eq_prove_round(m, bind, w.round, w.has_claim ? w.claim : nullptr, out_evals + i * JB_MAX_EVALS * 4);
             if (st != JB_OK) return st;
             m->rounds_done++;
@@ -1816,9 +1802,7 @@ static int overlapped_rounds(jb_scheduler* s, const jb_round_work* work, size_t 
             st = resident_consume(m->run, out, info);
             if (st == JB_RES_LOST) {  // recover (replays this round's bind), then an eval-only launch
                 st = resident_recover(m->run);
-                if (st == JB_OK) st = member_round(m, nullptr, true, nullptr);
-                if (st == JB_OK) st = wait_round_result0(c);
-                if (st == JB_OK) st = assemble_evals(c, m->m, true, c->h_result, w.claim, w.round, out_evals + i * JB_MAX_EVALS * 4);
+                if (st == JB_OK) st = launched_round(m, nullptr, true, w.claim, w.round, out_evals + i * JB_MAX_EVALS * 4);
             } else if (st == JB_OK) {
                 uint64_t vals[JB_MAX_EVALS * 4];
                 answer_values(m, info[0], out, vals);

@@ -96,11 +96,22 @@ struct SourceCol {
     uint32_t K = 0;
 };
 
+// What a member proves, fixed when it is created. The kind decides which pass serves a round, how many tables the
+// member reports and where their final values lie; eq weighting and index sharding are properties on top of it.
+enum class MemberKind {
+    Dense,       // a product or sum of products over field tables (also an expression that is exactly such a shape)
+    Expr,        // the expression pass over tables or sources (ex)
+    Product,     // the product of m <= 16 tables or sources (terms = 1) through product_round_kernel
+    ReadWrite,   // read-write checking (rw): sparse cycle rounds, then the expression pass over K-entry tables
+    Booleanity,  // booleanity (bl): address rounds, then cycle rounds
+};
+
 // One ProveRounds member on the device (~ Box<dyn SumcheckKernel>): the relation
 //   sum_x sum_{k<P} prod_{j<D} f_{kD+j}(x)       (degree D, T = D * P dense tables)
 // optionally weighted by a split eq polynomial, optionally index-sharded over ranks.
 struct jb_member {
     jb_ctx* ctx;
+    MemberKind kind = MemberKind::Dense;
     std::vector<Table> tables;
     int m;       // D: factors per term = degree of the (unweighted) relation
     int terms = 1;  // P
@@ -142,25 +153,23 @@ struct jb_member {
     // do not include it.
     bool pend = false;
     uint64_t pend_r[4];
-    // expression member (jb_member_create_expr): the summand is ex's weighted monomials over the tables (m = the
-    // largest monomial degree, `terms` unused); it never runs in a resident kernel
-    bool expr = false;
+    // Expr (jb_member_create_expr): the summand is ex's weighted monomials over the tables (m = the largest monomial
+    // degree, `terms` unused); also a ReadWrite member's address rounds
     jb::ExprParams ex;
-    // expression member over sources (jb_member_create_expr_sources): until the sources are bound, src[j] describes
-    // table j - a compact or one-hot source reads its member-owned column and its Table's buffer is where the bind
-    // writes the len/2 field entries. Cleared (and the columns released) by the bind.
+    // an Expr or Product member over sources (jb_member_create_*_sources): until the sources are bound, src[j]
+    // describes table j - a compact or one-hot source reads its member-owned column and its Table's buffer is where the
+    // bind writes the len/2 field entries. Cleared (and the columns released) by the bind.
     std::vector<SourceCol> src;
-    // product member over sources (jb_member_create_product_sources): the product of its m tables / sources, m <= 16
-    // (terms = 1), through product_round_kernel; src as for the expression member over sources
-    bool product = false;
-    // read-write checking member (jb_member_create_read_write): the sparse cycle phase until the last cycle variable is
-    // bound, then an expression member over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (expr set, rw released)
+    // ReadWrite (jb_member_create_read_write): the sparse cycle phase until the last cycle variable is bound, then the
+    // expression pass over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (RwState::cycles)
     struct RwState* rw = nullptr;
-    int ntables() const { return rw ? (int)tables.size() : expr ? ex.ntables : m * terms; }
-    // booleanity member (jb_member_create_booleanity): its d tables live in bl, not in `tables`, and ntables() does not
-    // count them (the entry points that report or read tables ask bl for d)
+    // Booleanity (jb_member_create_booleanity): its d tables live in bl, not in `tables`
     struct BoolState* bl = nullptr;
+    int ntables() const;  // the tables the member reports (final_evals, export_table)
 };
+
+// A new member with the fields every kind sets, and rounds = log2(len) (len a power of two); null when out of memory.
+jb_member* new_member(jb_ctx* c, MemberKind kind, int m, int terms, int order, size_t len);
 
 // The split-eq weight tables of a round (e_out[y >> in_bits] * e_in[y & mask]).
 struct EqWeights {
@@ -175,6 +184,7 @@ constexpr int RW_MAX_ACCESSES = JB_RW_MAX_ACCESSES;
 // buffers that take turns as the input and the output of a bind. Per entry and buffer: key and row (u32), the field
 // arrays ra_0 .. ra_{A-1}, val, vs (Val before the row's block of cycles) and ve (Val after it).
 struct RwState {
+    bool cycles = true;  // the cycle phase; cleared when the last cycle variable is bound and ex is the address phase's
     int A = 0, w = 0;
     uint64_t coeff[RW_MAX_ACCESSES][4];
     int d[RW_MAX_ACCESSES];
@@ -249,6 +259,7 @@ int bool_finish(jb_member* mem, const uint64_t r[4]);
 // Where ra_i's single entry lies once the member is fully bound.
 const uint64_t* bool_final_entry(const jb_member* mem, int i);
 void bool_release(jb_member* mem);
+inline int jb_member::ntables() const { return kind == MemberKind::Booleanity ? bl->d : (int)tables.size(); }
 
 // mle_eval.cu ------------------------------------------------------------------------------------------------
 // G_p[k] = sum_{j: addr_p(j) = k} eq(r_cycle, j) for count device address columns into out[p] (K elements each);
@@ -277,6 +288,9 @@ void sources_release(jb_member* mem);
 int sources_one_hot_eq(jb_ctx* c, SourceCol& s, size_t len, const uint64_t* r_addr, size_t log_k, unsigned int* d_flag);
 
 // resident.cu ------------------------------------------------------------------------------------------------
+// Whether a resident kernel may serve the member's kind: Dense without split-eq weighting (resident_eligible also
+// asks the member's current state).
+inline bool resident_kind(const jb_member* mem) { return mem->kind == MemberKind::Dense && !mem->eq; }
 // Starts a resident kernel serving `n` members (same D, P, order, same context; n <= RES_MAX_MEMBERS). Members
 // must be plain (not eq / sharded-with-tail). `exchange`: the kernel may be asked to all-reduce member 0's sums
 // over peer memory (sharded rounds). JB_ERR_UNSUPPORTED = not eligible (caller falls back to launches).

@@ -450,19 +450,14 @@ int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_k
     if (scale && !canonical_fr(scale)) return c->fail(JB_ERR_INVALID, "read-write: scale not canonical");
 
     // everything the rounds need is allocated here
-    jb_member* mem = new (std::nothrow) jb_member();
+    jb_member* mem = new_member(c, MemberKind::ReadWrite, 2, 1, JB_LOW_TO_HIGH, K * T);
     if (!mem) return JB_ERR_OOM;
     RwState* rw = new (std::nothrow) RwState();
     if (!rw) {
         delete mem;
         return JB_ERR_OOM;
     }
-    mem->ctx = c;
     mem->rw = rw;
-    mem->m = 2;
-    mem->order = JB_LOW_TO_HIGH;
-    mem->rounds = t + (size_t)log2_of(K);
-    mem->len = K * T;
     rw->A = (int)A;
     rw->w = (int)w;
     rw->T = T;

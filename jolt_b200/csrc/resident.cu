@@ -168,7 +168,7 @@ void release_run(ResidentRun* run, bool mark_no_resident) {
 }  // namespace
 
 bool resident_eligible(const jb_member* mem) {
-    if (!mem || !mem->ctx->use_tail || mem->eq || mem->expr || mem->product || mem->run) return false;
+    if (!mem || !mem->ctx->use_tail || !resident_kind(mem) || mem->run) return false;
     if (mem->len < 2 || (mem->len & (mem->len - 1))) return false;
     // a member whose big run had to make room for other work only re-enters service once its run is small
     if (mem->no_resident && mem->len > RES_SMALL_LEN) return false;

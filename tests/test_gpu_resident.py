@@ -156,7 +156,8 @@ def test_resident_run_survives_interleaved_context_work(sess):
 def test_lost_resident_kernel_is_recovered_with_launches(sess):
     """ADVICE r01: a resident kernel that stops waiting for commands (the host was held up - here a 3 ms device
     timeout and a host that sleeps) must not fail the member: the unexecuted binds are replayed with launches, the
-    round is recomputed, and the proof is the oracle's, both in thin (lookahead) and in generic rounds."""
+    round is recomputed, and the proof is the oracle's, both in thin (lookahead) and in generic rounds, and in a
+    scheduler batch whose short members run on their own small kernels."""
     import time
     os.environ["JB_RESIDENT_TIMEOUT_S"] = "0.003"
     try:
@@ -182,6 +183,25 @@ def test_lost_resident_kernel_is_recovered_with_launches(sess):
         gpu.finish_rounds(bind)
         assert gpu.final_evals() == [C.mont_to_ints(t)[0] for t in cur]
         gpu.close()
+    # a batch of two shapes (not one resident kernel): each member is on its own small run once it is short, and the
+    # host sleeps between rounds
+    shapes = [(3, 14, 0), (2, 9, 5)]
+    tabs, desc, total, max_vars = batch_fixture(shapes, 4100)
+    pts = O.synthetic_point(max_vars, 403)
+    want = O.prove_batch(desc, [O.ProductMember(t, LOW_TO_HIGH) for t in tabs], max_vars, 3, total, lambda r, c: pts[r])
+    mems = [ProductMember(s2, [Polynomial.from_ints(s2, t) for t in tb], LOW_TO_HIGH) for tb in tabs]
+
+    def draw(r, poly):
+        if r in (2, 6, 10, 13):
+            time.sleep(0.05)
+        return pts[r]
+
+    got = jolt_b200.prove_batch_native([BatchMember(**d) for d in desc], mems, max_vars, 3, total, draw)
+    assert got.challenges == want["challenges"] and got.final_claim == want["final_claim"]
+    assert [p.coefficients for p in got.round_polynomials] == want["round_polys"]
+    for mem, tb, d in zip(mems, tabs, desc):
+        assert mem.final_evals() == [O.evaluate(t, list(reversed(pts[d["offset"]:d["offset"] + d["rounds"]]))) for t in tb]
+        mem.close()
     s2.close()
 
 
