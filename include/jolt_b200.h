@@ -238,7 +238,8 @@ int jb_member_create_expr(jb_ctx* ctx, const jb_table* tables, size_t ntables, c
  *  - JB_SOURCE_COMPACT: `len` integers of `kind` (any jb_scalar_kind but JB_SCALAR_FR); value F::from(v).
  *  - JB_SOURCE_ONE_HOT: `len` addresses of `kind` (JB_SCALAR_U8 / U16; the all-ones value is the none value, as in
  *    jb_one_hot_evaluate); f(j) = eq(r_addr, addr[j]) with r_addr = log2 K canonical coordinates, r_addr[0] <-> the
- *    address MSB, and 0 for the none value. K a power of two, 1 <= K <= 2^16.
+ *    address MSB, and 0 for the none value. K a power of two, 1 <= K <= 2^16. (Product members over sources also
+ *    take JB_SCALAR_U32 addresses; expression members refuse them with JB_ERR_INVALID.)
  * `values` and `r_addr` are borrowed for the call (on_device = 0: host memory; 1: caller-owned device memory): the
  * columns are copied into member-owned device memory and each one-hot source's eq(r_addr, .) table (K entries) is built
  * at creation, together with every buffer the member's rounds need, so JB_ERR_OOM can only arise here. The copies
@@ -273,7 +274,11 @@ int jb_member_create_expr_sources(jb_ctx* ctx, const jb_source* sources, size_t 
  * legacy subprotocols/mles_product_sum.rs), which no sum of smaller members can express. Each f_i is a jb_source with
  * exactly the semantics, ownership, on-device rules and checks of jb_member_create_expr_sources (table sources owned
  * by the member, columns copied at creation, everything the rounds need allocated here so JB_ERR_OOM can only arise
- * here, a bad address found on the device at creation with nothing left allocated).
+ * here, a bad address found on the device at creation with nothing left allocated), with one difference: a one-hot
+ * source may also have JB_SCALAR_U32 addresses (none value 0xFFFFFFFF), with K a power of two, 1 <= K <= 2^24
+ * (JB_ERR_INVALID beyond), so RAM-sized address spaces (value evaluation inc * wa * LT, the final-value relation
+ * inc * wa) are products over their u32 write column. Each such source holds a K-entry eq table (32 K bytes,
+ * 512 MiB at K = 2^24) until round 1 binds it.
  *  - degree = d, + 1 with eq_w_or_null (nvars = log2 len elements, w[0] <-> the most significant index bit, optional
  *    scale): jb_member_prove_round writes degree + 1 evaluations (up to 18). With eq the running claim is mandatory
  *    in prove_round, a zero eq factor at the current variable is refused and jb_eq_member_scalar returns
@@ -297,9 +302,12 @@ int jb_member_create_product_sources(jb_ctx* ctx, const jb_source* sources, size
  * access a = 0 .. A-1 (1 <= A <= JB_RW_MAX_ACCESSES) reads its address column addr_a, its value column v_a, its
  * coefficient c_a and its flag d_a in {0, 1}; access w is the write. Two accesses may share an address column: RAM is
  * one column used twice, (c = 1, d = 0) for the read and (c = gamma, d = 1) for the write; registers are rs1, rs2, rd.
- *  - T = 2^t cycles, 2 <= T <= 2^30; K = 2^kappa addresses, 1 <= K <= 2^16; min(K, distinct address columns) * T <
- *    2^31. Address columns: T entries of addr_kind (JB_SCALAR_U8 / U16; the all-ones value means no access), all in
- *    host memory or all in device memory (addr_on_device), aligned to their entry.
+ *  - T = 2^t cycles, 2 <= T <= 2^30; K = 2^kappa addresses, 1 <= K <= 2^16 for addr_kind JB_SCALAR_U8 / U16 and
+ *    1 <= K <= 2^24 for JB_SCALAR_U32 (RAM's word addresses; JB_ERR_INVALID beyond); min(K, distinct address columns)
+ *    * T < 2^31. Address columns: T entries of addr_kind (the all-ones value of the width means no access), all in
+ *    host memory or all in device memory (addr_on_device), aligned to their entry. The address phase holds A + 2
+ *    K-entry tables with their half-size ping-pong buffers and the K-entry init: about (1.5 (A + 2) + 1) * 32 K bytes,
+ *    4 GiB for RAM (A = 2) at K = 2^24.
  *  - Values (T entries), inc (T entries) and init (K entries) are jb_sources of type JB_SOURCE_TABLE (a field table,
  *    left to the caller) or JB_SOURCE_COMPACT (a compact column of any jb_scalar_kind but JB_SCALAR_FR, e.g. inc as
  *    i64 / i128 / S64 / S128). Every column and table is borrowed for the call only.
@@ -551,7 +559,7 @@ int jb_msm_g1_one_hot_rows(jb_ctx* ctx, jb_srs bases, const void* const* columns
  * is allocated: JB_ERR_INVALID for a null pointer, an unknown kind or layout, a length, T or K that is not a power of
  * two, tables of different lengths, nvars != log2(length), non-canonical point limbs, and - found on the device, the
  * context stays usable - a one-hot address >= K that is not the none value. JB_ERR_UNSUPPORTED beyond the limits:
- * nvars <= 40; one-hot T < 2^31 and K <= 2^16. count == 0 -> JB_OK.
+ * nvars <= 40; one-hot T < 2^31 and K <= 2^16 (K <= 2^24 for JB_SCALAR_U32 columns). count == 0 -> JB_OK.
  *
  * Resident tables of length 2^nvars (bound ones included), which are not modified: out[i] = tables[i] at point. */
 int jb_table_evaluate_batch(jb_ctx* ctx, const jb_table* tables, size_t count, const uint64_t* point, size_t nvars,
@@ -561,8 +569,9 @@ int jb_table_evaluate_batch(jb_ctx* ctx, const jb_table* tables, size_t count, c
  * jb_table_upload_small); 1: device pointers owned by the caller (e.g. torch tensors), read in place. */
 int jb_small_evaluate_batch(jb_ctx* ctx, const void* const* columns, size_t count, const int* kinds, size_t len,
                             int on_device, const uint64_t* point, size_t nvars, uint64_t* out);
-/* One-hot polynomials: the 0/1 polynomial jb_msm_g1_one_hot_rows commits (same kinds, none value, layouts and flat
- * index), from count address columns of T entries. point: log2(K T) coordinates; JB_ONE_HOT_CYCLE_MAJOR:
+/* One-hot polynomials: the 0/1 polynomial jb_msm_g1_one_hot_rows commits (same none value, layouts and flat index),
+ * from count address columns of T entries of `kind`: JB_SCALAR_U8 / U16 as there, or JB_SCALAR_U32 (none value
+ * 0xFFFFFFFF) for address spaces up to K = 2^24, such as RAM's; the K-entry eq(r_addr, .) table is 32 K bytes. point: log2(K T) coordinates; JB_ONE_HOT_CYCLE_MAJOR:
  * r_cycle = point[0 .. log T), r_addr = the rest; JB_ONE_HOT_ADDRESS_MAJOR: r_addr first.
  *   out[p] = sum_{j: addr_p[j] != none} eq(r_cycle, j) eq(r_addr, addr_p[j]). */
 int jb_one_hot_evaluate(jb_ctx* ctx, const void* const* columns, size_t count, int kind, size_t T, size_t K, int layout,
@@ -570,7 +579,8 @@ int jb_one_hot_evaluate(jb_ctx* ctx, const void* const* columns, size_t count, i
 /* The pushforward of eq(r_cycle, .) through each address column (r_cycle: log2 T coordinates): count NEW resident
  * tables of K entries, G_p[k] = sum_{j: addr_p[j] = k} eq(r_cycle, j) - the cycle-major polynomial bound HighToLow by
  * r_cycle, so sum_k eq(r_addr, k) G_p[k] is jb_one_hot_evaluate's value. Ordinary tables: they feed the product and
- * expression members (the address phase of a one-hot read-checking sumcheck). Nothing is created on an error. */
+ * expression members (the address phase of a one-hot read-checking sumcheck). Kinds and limits as jb_one_hot_evaluate;
+ * K > 512 bins in global memory, 64 K bytes of lanes per column during the call. Nothing is created on an error. */
 int jb_one_hot_pushforward(jb_ctx* ctx, const void* const* columns, size_t count, int kind, size_t T, size_t K,
                            int on_device, const uint64_t* r_cycle, jb_table* out_tables);
 

@@ -418,28 +418,38 @@ def evaluate_small(session: Session, columns, point, kinds=None) -> list[int]:
     return F.limbs_to_ints(out)
 
 
-def _address_columns(columns, what: str):
+def _address_columns(columns, what: str, u32: bool = False):
     """(pointers, kind, T, on_device, keep-alive) for one-hot address columns: uint8 / uint16 numpy arrays or CUDA
-    tensors (torch.uint8, torch.uint16, or torch.int16 read as raw 16-bit words), all of one dtype and length."""
+    tensors (torch.uint8, torch.uint16, or torch.int16 read as raw 16-bit words), all of one dtype and length. With
+    `u32` (the entry points that take RAM-sized address spaces, K up to 2^24) also uint32 arrays and torch.int32 /
+    torch.uint32 tensors, read as raw 32-bit words (0xFFFFFFFF, i.e. int32 -1, is the none value)."""
     if isinstance(columns, np.ndarray) and columns.ndim == 1 or _is_device_tensor(columns):
         columns = [columns]
     columns = list(columns)
     if not columns:
         return [], SCALAR_KINDS["u8"], 1, 0, []
+    widths = "uint8 or 16-bit" + (" or 32-bit" if u32 else "")
     if all(_is_device_tensor(c) for c in columns):
         import torch
-        u16 = {torch.int16} | ({torch.uint16} if hasattr(torch, "uint16") else set())
+        kinds = {torch.uint8: "u8", torch.int16: "u16"}
+        if hasattr(torch, "uint16"):
+            kinds[torch.uint16] = "u16"
+        if u32:
+            kinds[torch.int32] = "u32"
+            if hasattr(torch, "uint32"):
+                kinds[torch.uint32] = "u32"
         dt = columns[0].dtype
-        if (dt != torch.uint8 and dt not in u16) or any(c.dtype != dt or c.dim() != 1 or not c.is_contiguous()
-                                                        or c.numel() != columns[0].numel() for c in columns):
-            raise ValueError(f"{what}: columns must be contiguous 1-D uint8 or 16-bit tensors of one dtype and length")
-        kind = SCALAR_KINDS["u8" if dt == torch.uint8 else "u16"]
-        return [c.data_ptr() for c in columns], kind, columns[0].numel(), 1, columns
+        if dt not in kinds or any(c.dtype != dt or c.dim() != 1 or not c.is_contiguous()
+                                  or c.numel() != columns[0].numel() for c in columns):
+            raise ValueError(f"{what}: columns must be contiguous 1-D {widths} tensors of one dtype and length")
+        return [c.data_ptr() for c in columns], SCALAR_KINDS[kinds[dt]], columns[0].numel(), 1, columns
     cols = [np.ascontiguousarray(c) for c in columns]
     dt = cols[0].dtype
-    if dt not in ONE_HOT_NONE or any(c.dtype != dt or c.ndim != 1 or c.shape != cols[0].shape for c in cols):
-        raise ValueError(f"{what}: columns must be 1-D uint8 or uint16 arrays of one dtype and length")
-    kind = SCALAR_KINDS["u8" if dt == np.uint8 else "u16"]
+    if (dt not in ONE_HOT_NONE or (dt == np.uint32 and not u32)
+            or any(c.dtype != dt or c.ndim != 1 or c.shape != cols[0].shape for c in cols)):
+        raise ValueError(f"{what}: columns must be 1-D uint8 or uint16{' or uint32' if u32 else ''} arrays of one dtype "
+                         "and length")
+    kind = SCALAR_KINDS[{1: "u8", 2: "u16", 4: "u32"}[dt.itemsize]]
     return [c.ctypes.data for c in cols], kind, cols[0].shape[0], 0, cols
 
 
@@ -450,7 +460,7 @@ def one_hot_evaluate(session: Session, columns, K: int, point, layout: str = "cy
     an address. "cycle_major": r_cycle = point[:log T], r_addr = the rest; "address_major" the other way round."""
     if layout not in ONE_HOT_LAYOUTS:
         raise ValueError(f"one_hot_evaluate: layout must be one of {sorted(ONE_HOT_LAYOUTS)}")
-    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_evaluate")
+    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_evaluate", u32=True)
     if not ptrs:
         return []
     pt = point_limbs(point)
@@ -468,7 +478,7 @@ def one_hot_pushforward(session: Session, columns, K: int, r_cycle) -> list[Poly
     """G[k] = sum_{j: column[j] = k} eq(r_cycle, j) for each address column (jb_one_hot_pushforward): new device
     polynomials of K entries - the cycle-major one-hot polynomial bound HighToLow by r_cycle (log2 T coordinates),
     ready for the address phase of a read-checking sumcheck (ProductMember / ExpressionMember)."""
-    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_pushforward")
+    ptrs, kind, T, dev, _keep = _address_columns(columns, "one_hot_pushforward", u32=True)
     if not ptrs:
         return []
     pt = point_limbs(r_cycle)
@@ -952,8 +962,8 @@ class ReadWriteCheckingMember(ExpressionMember):
       sum_{k<K} sum_{j<T} scale * eq(w_cycle, j) * sum_a c_a * ra_a(k, j) * (Val(k, j) + d_a * inc(j))
     over the sparse K x T memory matrix, from the witness columns, in O(A T) memory. ra_a(k, j) = [addr_a(j) = k];
     Val(k, j) = init(k) + the increments of the earlier cycles whose write address is k. `accesses`: up to 4 tuples
-    (addresses, values, coeff, d) - a uint8 / uint16 address column (the all-ones value = no access; accesses may share
-    one column), the values v_a(j) = Val(addr_a(j), j) the witness holds (a Source.table or Source.compact, or anything
+    (addresses, values, coeff, d) - a uint8 / uint16 address column, K <= 2^16, or a uint32 one, K <= 2^24 (the all-ones
+    value = no access; accesses may share one column), the values v_a(j) = Val(addr_a(j), j) the witness holds (a Source.table or Source.compact, or anything
     Source.compact takes), c_a (an int or 4 Montgomery limbs) and d_a in {0, 1}; access `write` is the write. `inc`
     (T entries) and `init` (K entries) likewise. Everything is borrowed for the call. Degree 3, log2 T + log2 K rounds,
     LowToHigh only; the running claim is mandatory. final_evals() returns ra_0 .. ra_{A-1}, Val, inc at the point."""
@@ -962,7 +972,7 @@ class ReadWriteCheckingMember(ExpressionMember):
                  order: int = LOW_TO_HIGH):
         def src(x):
             return x if isinstance(x, Source) else Source.compact(x)
-        ptrs, kind, T, dev, keep = _address_columns([a[0] for a in accesses], "ReadWriteCheckingMember")
+        ptrs, kind, T, dev, keep = _address_columns([a[0] for a in accesses], "ReadWriteCheckingMember", u32=True)
         arr = (_lib.RwAccessC * max(len(accesses), 1))()
         for i, (_addr, values, coeff, d) in enumerate(accesses):
             arr[i].addr = ptrs[i]
@@ -1059,9 +1069,11 @@ class Source:
     @classmethod
     def one_hot(cls, addresses, K: int, r_addr) -> "Source":
         """The one-hot polynomial ra(r_addr, j) = eq(r_addr, addresses[j]) (0 where the column holds the none value,
-        the all-ones value of its width): a uint8 / uint16 numpy array or CUDA tensor, K a power of two, r_addr
-        log2 K coordinates (r_addr[0] <-> the address MSB)."""
-        ptrs, kind, T, dev, keep = _address_columns(addresses, "Source.one_hot")
+        the all-ones value of its width): a uint8 / uint16 numpy array or CUDA tensor, K a power of two <= 2^16, r_addr
+        log2 K coordinates (r_addr[0] <-> the address MSB). ProductMember.from_sources also takes a uint32 column
+        (numpy uint32, torch.int32 / torch.uint32 read as raw words) with K <= 2^24; ExpressionMember.from_sources
+        refuses it (JB_ERR_INVALID)."""
+        ptrs, kind, T, dev, keep = _address_columns(addresses, "Source.one_hot", u32=True)
         if len(ptrs) != 1:
             raise ValueError("Source.one_hot: one address column")
         r = point_limbs(r_addr)
@@ -1261,7 +1273,7 @@ def prove_batch_native(members_desc: list[BatchMember], members: list[ProductMem
 # ---- G1 / MSM ---------------------------------------------------------------------------------------
 # One-hot address columns (G1Bases.one_hot_rows): the entry value that means "this cycle touched no address" (RAM's
 # None), per column dtype, and the coefficient layouts of include/jolt_b200.h.
-ONE_HOT_NONE = {np.dtype(np.uint8): 0xFF, np.dtype(np.uint16): 0xFFFF}
+ONE_HOT_NONE = {np.dtype(np.uint8): 0xFF, np.dtype(np.uint16): 0xFFFF, np.dtype(np.uint32): 0xFFFFFFFF}
 ONE_HOT_LAYOUTS = {"cycle_major": 0, "address_major": 1}
 
 

@@ -973,8 +973,9 @@ int jb_member_create_expr(jb_ctx* c, const jb_table* handles, size_t ntables, co
 }
 
 // ---- expression member over sources ---------------------------------------------------------------------
-// The checks on one source (context lock held). log_k: log2 K of a one-hot source.
-static int check_source(jb_ctx* c, const jb_source& sr, size_t len, size_t* log_k) {
+// The checks on one source (context lock held). log_k: log2 K of a one-hot source. Product members take u32 address
+// columns (K <= 2^24), expression members u8 / u16 (K <= 2^16): widest is the widest address kind of the member.
+static int check_source(jb_ctx* c, const jb_source& sr, size_t len, int widest, size_t* log_k) {
     if (sr.type == JB_SOURCE_TABLE) {
         const Table* t = c->find(sr.table);
         if (!t) return c->fail(JB_ERR_INVALID, "expr sources: unknown table handle");
@@ -984,9 +985,11 @@ static int check_source(jb_ctx* c, const jb_source& sr, size_t len, size_t* log_
     if (sr.type != JB_SOURCE_COMPACT && sr.type != JB_SOURCE_ONE_HOT)
         return c->fail(JB_ERR_INVALID, "expr sources: unknown source type");
     if (sr.type == JB_SOURCE_COMPACT) return check_compact_column(c, "expr sources", sr.kind, sr.values, sr.on_device);
-    // (here a K above 2^16 is invalid, not unsupported)
-    if (sr.K > ((size_t)1 << 16)) return c->fail(JB_ERR_INVALID, "expr sources: K must be a power of two in [1, 2^16]");
-    const int st = check_one_hot_columns(c, "expr sources", sr.kind, len, sr.K, sr.on_device, &sr.values, 1);
+    // (here a K above the kind's limit is invalid, not unsupported)
+    if (one_hot_kind(sr.kind, widest) && sr.K > one_hot_max_k(sr.kind))
+        return c->fail(JB_ERR_INVALID, sr.kind == SK_U32 ? "product sources: K must be a power of two in [1, 2^24]"
+                                                         : "expr sources: K must be a power of two in [1, 2^16]");
+    const int st = check_one_hot_columns(c, "expr sources", sr.kind, len, sr.K, sr.on_device, &sr.values, 1, widest);
     if (st != JB_OK) return st;
     *log_k = (size_t)log2_of(sr.K);
     if (*log_k && !sr.r_addr) return c->fail(JB_ERR_INVALID, "expr sources: null r_addr");
@@ -1022,7 +1025,8 @@ static int create_over_sources(jb_ctx* c, MemberKind kind, const jb_source* sour
             return c->fail(JB_ERR_INVALID, "expr member: point length must equal log2(table length) >= 1");
         size_t log_k[JB_PRODUCT_MAX_FACTORS] = {0};
         for (size_t i = 0; i < nsources; ++i) {
-            if ((st = check_source(c, sources[i], len, &log_k[i])) != JB_OK) return st;
+            if ((st = check_source(c, sources[i], len, kind == MemberKind::Product ? SK_U32 : SK_U16, &log_k[i])) != JB_OK)
+                return st;
             for (size_t k = 0; k < i; ++k)
                 if (sources[i].type == JB_SOURCE_TABLE && sources[k].type == JB_SOURCE_TABLE && sources[k].table == sources[i].table)
                     return c->fail(JB_ERR_INVALID, "member: duplicate table handle");

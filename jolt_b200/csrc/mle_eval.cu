@@ -13,6 +13,9 @@
 // of 32-bit limb sums (REDUX over each warp, one atomic per lane per block); jb_wide_lanes_reduce_host folds the
 // lanes. Integer lane sums are exact and order-free: results are bit-exact and deterministic whatever the schedule.
 //
+// One-hot columns are u8, u16 or u32 (columns.cuh). The u8 instances read bytes; the 16-bit instances also serve u32
+// columns, reading the width from the launch's kind (a uniform branch), so K up to 2^24 costs no more instances.
+//
 // Compact values are plain integers, not Montgomery values: sum e~ v (e~ = e R) is already R * sum e v, so the lanes
 // fold to the plain integer value of the sum and the host multiplies by R^2 once (a Montgomery product) to get its
 // Montgomery form. A negative value accumulates (p - e~) |v|.
@@ -52,18 +55,20 @@ struct EvalCol {  // one output of a launch: its source and its lane block
 
 // ---- value loaders: A += e * v(i) (field and compact values: value_src.cuh) ------------------------------------
 // v_j = eq(r_addr, addr_j), 0 for the none value; an address >= K that is not none raises *bad and counts as 0.
+// KIND is SK_U8, or SK_U16 for the instance that reads `kind` (SK_U16 / SK_U32) at run time.
 template <int KIND, bool SMEM>
 struct OneHotSrc {
     static constexpr int SMEM_U4 = SMEM ? 2 * OH_SMEM_K : 1;
     const uint64_t* eq_addr;
     uint32_t K;
     unsigned int* bad;
+    int kind;
     __device__ void init(uint4* s) const {
         if (SMEM)
             for (uint32_t i = threadIdx.x; i < 2 * K; i += blockDim.x) s[i] = reinterpret_cast<const uint4*>(eq_addr)[i];
     }
     __device__ __forceinline__ void acc(uint32_t (&A)[17], const Fr& e, const void* p, size_t i, const uint4* s) const {
-        const uint32_t a = ld_address(p, i, KIND);
+        const uint32_t a = ld_address<SK_U32>(p, i, KIND == SK_U8 ? SK_U8 : kind);
         if (a == NO_ADDRESS) return;
         if (a >= K) {
             atomicOr(bad, 1u);
@@ -118,11 +123,38 @@ __global__ void __launch_bounds__(EV_BLOCK, 2)
     }
 }
 
-// lanes: count x K x 8 (zeroed); the grid is that of mle_eval_kernel over the T cycles.
+// One thread's walk over rows [h0, h1) of its column l of an address column of kind LK: runs of one address are summed
+// in acc and flushed into bins when the address changes (cur, acc: the open run, flushed by the caller).
+template <int LK>
+__device__ __forceinline__ void pf_walk(const void* p, size_t h0, size_t h1, size_t L, size_t l, const Fr& el,
+                                        const uint64_t* e_hi, uint32_t K, unsigned int* bad, unsigned long long* bins,
+                                        int lane, uint32_t& cur, Fr& acc) {
+    for (size_t h = h0; h < h1; ++h) {  // block-uniform trip count: the warp stays converged for pf_flush
+        uint32_t a = NO_KEY;
+        Fr w;
+        if (l < L) {
+            a = ld_address<SK_U32>(p, h * L + l, LK);  // the none value is NO_KEY (>= K)
+            if (a < K) {
+                w = fp_mul(ld_elem<Fr>(e_hi, h), el);
+            } else if (a != NO_KEY) {
+                atomicOr(bad, 1u);
+                a = NO_KEY;
+            }
+        }
+        pf_flush(a != NO_KEY && cur != NO_KEY && a != cur, cur, acc, bins, lane);
+        if (a != NO_KEY) {
+            acc = a == cur ? fp_add(acc, w) : w;
+            cur = a;
+        }
+    }
+}
+
+// lanes: count x K x 8 (zeroed); the grid is that of mle_eval_kernel over the T cycles. KIND as in OneHotSrc; the
+// 16-bit instance picks its walk by `kind` once per column, so the walk itself loads one width.
 template <int KIND, bool SMEM>
 __global__ void __launch_bounds__(EV_BLOCK)
     pushforward_kernel(const EvalCol* cols, size_t count, const uint64_t* e_hi, const uint64_t* e_lo, int n_lo,
-                       size_t rows, size_t rpb, uint32_t K, unsigned long long* lanes, unsigned int* bad) {
+                       size_t rows, size_t rpb, uint32_t K, int kind, unsigned long long* lanes, unsigned int* bad) {
     __shared__ unsigned long long s_bins[SMEM ? PF_SMEM_K * 8 : 1];
     const int tid = threadIdx.x, lane = tid & 31;
     const size_t L = (size_t)1 << n_lo;
@@ -139,24 +171,9 @@ __global__ void __launch_bounds__(EV_BLOCK)
         const void* p = cols[z].ptr;
         uint32_t cur = NO_KEY;  // the thread's run: address and the field sum of its weights
         Fr acc = Fr::zero();
-        for (size_t h = h0; h < h1; ++h) {  // block-uniform trip count: the warp stays converged for pf_flush
-            uint32_t a = NO_KEY;
-            Fr w;
-            if (l < L) {
-                a = ld_address(p, h * L + l, KIND);  // the none value is NO_KEY (>= K)
-                if (a < K) {
-                    w = fp_mul(ld_elem<Fr>(e_hi, h), el);
-                } else if (a != NO_KEY) {
-                    atomicOr(bad, 1u);
-                    a = NO_KEY;
-                }
-            }
-            pf_flush(a != NO_KEY && cur != NO_KEY && a != cur, cur, acc, bins, lane);
-            if (a != NO_KEY) {
-                acc = a == cur ? fp_add(acc, w) : w;
-                cur = a;
-            }
-        }
+        if (KIND == SK_U8) pf_walk<SK_U8>(p, h0, h1, L, l, el, e_hi, K, bad, bins, lane, cur, acc);
+        else if (kind == SK_U32) pf_walk<SK_U32>(p, h0, h1, L, l, el, e_hi, K, bad, bins, lane, cur, acc);
+        else pf_walk<SK_U16>(p, h0, h1, L, l, el, e_hi, K, bad, bins, lane, cur, acc);
         pf_flush(cur != NO_KEY, cur, acc, bins, lane);
         if (SMEM) {
             __syncthreads();
@@ -279,7 +296,7 @@ int one_hot_pushforward_into(jb_ctx* c, const void* const* dev_columns, size_t c
         const bool sm = K <= PF_SMEM_K;
 #define JB_PF_LAUNCH(KD, SM)                                                                                       \
     pushforward_kernel<KD, SM><<<p.grid, EV_BLOCK, 0, c->stream>>>(p.d_cols, count, p.e_hi(), p.e_lo(), p.n_lo, p.rows, \
-                                                                    p.rpb, (uint32_t)K, p.d_lanes, p.bad())
+                                                                    p.rpb, (uint32_t)K, kind, p.d_lanes, p.bad())
         if (kind == SK_U8) { if (sm) JB_PF_LAUNCH(SK_U8, true); else JB_PF_LAUNCH(SK_U8, false); }
         else { if (sm) JB_PF_LAUNCH(SK_U16, true); else JB_PF_LAUNCH(SK_U16, false); }
 #undef JB_PF_LAUNCH
@@ -360,7 +377,7 @@ int jb_small_evaluate_batch(jb_ctx* c, const void* const* columns, size_t count,
 int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K, int layout,
                         int on_device, const uint64_t* point, uint64_t* out) {
     if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;
-    int st = check_one_hot_columns(c, "one_hot_evaluate", kind, T, K, on_device, columns, count);
+    int st = check_one_hot_columns(c, "one_hot_evaluate", kind, T, K, on_device, columns, count, SK_U32);
     if (st != JB_OK) return st;
     if (layout != JB_ONE_HOT_CYCLE_MAJOR && layout != JB_ONE_HOT_ADDRESS_MAJOR)
         return c->fail(JB_ERR_INVALID, "one_hot_evaluate: unknown layout");
@@ -384,10 +401,10 @@ int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int
     if (st == JB_OK) st = p.begin(r_cycle, log_t, 17);
     if (st == JB_OK) {
         const bool sm = K <= OH_SMEM_K;
-        if (kind == SK_U8) st = sm ? launch_eval(p, OneHotSrc<SK_U8, true>{d_eq, (uint32_t)K, p.bad()}, 0, count)
-                                   : launch_eval(p, OneHotSrc<SK_U8, false>{d_eq, (uint32_t)K, p.bad()}, 0, count);
-        else st = sm ? launch_eval(p, OneHotSrc<SK_U16, true>{d_eq, (uint32_t)K, p.bad()}, 0, count)
-                     : launch_eval(p, OneHotSrc<SK_U16, false>{d_eq, (uint32_t)K, p.bad()}, 0, count);
+        if (kind == SK_U8) st = sm ? launch_eval(p, OneHotSrc<SK_U8, true>{d_eq, (uint32_t)K, p.bad(), kind}, 0, count)
+                                   : launch_eval(p, OneHotSrc<SK_U8, false>{d_eq, (uint32_t)K, p.bad(), kind}, 0, count);
+        else st = sm ? launch_eval(p, OneHotSrc<SK_U16, true>{d_eq, (uint32_t)K, p.bad(), kind}, 0, count)
+                     : launch_eval(p, OneHotSrc<SK_U16, false>{d_eq, (uint32_t)K, p.bad(), kind}, 0, count);
     }
     if (st == JB_OK) st = p.finish(out, nullptr);
     c->dev_free(d_eq);
@@ -397,7 +414,7 @@ int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int
 int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, int kind, size_t T, size_t K,
                            int on_device, const uint64_t* r_cycle, jb_table* out_tables) {
     if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;
-    int st = check_one_hot_columns(c, "one_hot_pushforward", kind, T, K, on_device, columns, count);
+    int st = check_one_hot_columns(c, "one_hot_pushforward", kind, T, K, on_device, columns, count, SK_U32);
     if (st != JB_OK) return st;
     const size_t log_t = (size_t)log2_of(T);
     if (count && !out_tables) return c->fail(JB_ERR_INVALID, "one_hot_pushforward: null pointer");

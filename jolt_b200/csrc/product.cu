@@ -44,6 +44,7 @@ enum : uint8_t { PROD_LEAF = 0, PROD_MERGE = 1 };
 // The kernel parameter: tables, sources and the evaluation program of the member (every existing pass keeps its own
 // 8-table structs). Node slots are 8 words each in the thread's column.
 struct ProductParams {
+    static constexpr int ADDRESS_WIDEST = SK_U32;  // product members over sources: u8 / u16 / u32 addresses
     const uint64_t* in[PROD_MAX];   // field tables (null for a source read from its column)
     uint64_t* out[PROD_MAX];        // bind destinations
     const uint64_t* e_out;          // WEIGHTED: the split-eq weight e_out[y >> in_bits] * e_in[y & mask]

@@ -213,7 +213,7 @@ __device__ __forceinline__ int cycle_keys(const RwCols& cols, size_t j, uint32_t
     aw = NO_ADDRESS;
 #pragma unroll
     for (int a = 0; a < A; ++a) {
-        ad[a] = ld_address(cols.addr[a], j, cols.addr_kind);
+        ad[a] = ld_address<SK_U32>(cols.addr[a], j, cols.addr_kind);
         if (ad[a] != NO_ADDRESS && ad[a] >= K) {
             if (bad) atomicOr(bad, RW_BAD_ADDRESS);
             ad[a] = NO_ADDRESS;
@@ -425,10 +425,12 @@ int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_k
     if (w >= A) return c->fail(JB_ERR_INVALID, "read-write: the write access is not an access");
     if (!pow2(T) || T < 2 || T > ((size_t)1 << 30))
         return c->fail(JB_ERR_INVALID, "read-write: T must be a power of two in [2, 2^30]");
-    if (!pow2(K) || K > ((size_t)1 << 16)) return c->fail(JB_ERR_INVALID, "read-write: K must be a power of two in [1, 2^16]");
+    if (!pow2(K) || (one_hot_kind(addr_kind, SK_U32) && K > one_hot_max_k(addr_kind)))
+        return c->fail(JB_ERR_INVALID, addr_kind == SK_U32 ? "read-write: K must be a power of two in [1, 2^24]"
+                                                           : "read-write: K must be a power of two in [1, 2^16]");
     const void* cols[RW_MAX_ACCESSES];
     for (size_t a = 0; a < A; ++a) cols[a] = acc[a].addr;
-    int st = check_one_hot_columns(c, what, addr_kind, T, K, addr_on_device, cols, A);
+    int st = check_one_hot_columns(c, what, addr_kind, T, K, addr_on_device, cols, A, SK_U32);
     if (st != JB_OK) return st;
     size_t ncols = 0;  // distinct address columns: a cycle has at most that many entries
     for (size_t a = 0; a < A; ++a) {

@@ -26,6 +26,7 @@ constexpr size_t SRC_SMEM_MAX = expr_smem_bytes(EXPR_MAX_TABLES) + (size_t)EXPR_
 
 // What the pass reads for each table j of the member. The type of a table is uniform over the grid.
 struct SourceParams {
+    static constexpr int ADDRESS_WIDEST = SK_U16;  // expression members over sources: u8 / u16 addresses
     const void* values[EXPR_MAX_TABLES];  // COMPACT / ONE_HOT column
     const uint64_t* eq[EXPR_MAX_TABLES];  // ONE_HOT: eq(r_addr, .) in global memory
     uint32_t K[EXPR_MAX_TABLES];
@@ -116,12 +117,13 @@ __global__ void __launch_bounds__(EXPR_BLOCK, 4)
     round_epilogue<EXPR_MAX_POINTS>(acc, red, out);
 }
 
-// Flags an address >= K that is not the none value.
-template <class A>
-__global__ void __launch_bounds__(256) check_addresses_kernel(const A* addr, size_t n, uint32_t K, unsigned int* bad) {
+// Flags an address >= K that is not the none value. U8: a u8 column; else `kind` (SK_U16 / SK_U32) at run time.
+template <bool U8>
+__global__ void __launch_bounds__(256) check_addresses_kernel(const void* addr, size_t n, int kind, uint32_t K,
+                                                              unsigned int* bad) {
     bool b = false;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t a = ld_address(addr, i, sizeof(A) == 1 ? SK_U8 : SK_U16);
+        const uint32_t a = ld_address<SK_U32>(addr, i, U8 ? SK_U8 : kind);
         b |= a != NO_ADDRESS && a >= K;
     }
     if (b) atomicOr(bad, 1u);
@@ -209,9 +211,9 @@ int sources_one_hot_eq(jb_ctx* c, SourceCol& sc, size_t len, const uint64_t* r_a
     if (st != JB_OK) return st;
     const unsigned grid = launch_grid(c, len, 256, 8);
     if (sc.kind == SK_U8)
-        check_addresses_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint8_t*>(sc.values), len, sc.K, d_flag);
+        check_addresses_kernel<true><<<grid, 256, 0, c->stream>>>(sc.values, len, sc.kind, sc.K, d_flag);
     else
-        check_addresses_kernel<<<grid, 256, 0, c->stream>>>(static_cast<const uint16_t*>(sc.values), len, sc.K, d_flag);
+        check_addresses_kernel<false><<<grid, 256, 0, c->stream>>>(sc.values, len, sc.kind, sc.K, d_flag);
     c->launches++;
     return c->check(cudaGetLastError(), "check_addresses_kernel launch");
 }

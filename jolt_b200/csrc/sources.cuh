@@ -1,7 +1,9 @@
 // The per-entry load of a member's source before its bind and the terminal bind from the columns, shared by the
 // passes that read sources in their own format (sources.cu, product.cu). A pass's parameter struct SP carries, per
 // table j: values[j] (the COMPACT / ONE_HOT column), eq[j] (ONE_HOT: eq(r_addr, .) in global memory), K[j], smem[j] (ONE_HOT: word offset of the eq
-// table staged in dynamic shared memory, or SRC_NO_SMEM), type[j] (JB_SOURCE_*) and kind[j].
+// table staged in dynamic shared memory, or SRC_NO_SMEM), type[j] (JB_SOURCE_*) and kind[j], and SP::ADDRESS_WIDEST,
+// the widest address kind its one-hot sources may have (columns.cuh): SK_U16 for the expression pass, whose source
+// pass sits at the register budget, SK_U32 for the product pass, so product members reach RAM-sized K.
 #pragma once
 #include <cstring>
 
@@ -22,7 +24,7 @@ __device__ __forceinline__ Fr src_value(const SP& sp, int j, size_t i, const uin
         const bool neg = ld_small(sp.values[j], i, sp.kind[j], mag);
         return promote_small(mag, neg);
     }
-    const uint32_t a = ld_address(sp.values[j], i, sp.kind[j]);
+    const uint32_t a = ld_address<SP::ADDRESS_WIDEST>(sp.values[j], i, sp.kind[j]);
     if (a >= sp.K[j]) return Fr::zero();  // none (NO_ADDRESS; creation refused any other a >= K)
     if (sp.smem[j] != SRC_NO_SMEM) {
         const uint4* s = reinterpret_cast<const uint4*>(dsm + sp.smem[j]);

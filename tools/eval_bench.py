@@ -3,7 +3,8 @@ and jb_one_hot_pushforward against the route callers had before them - clone (or
 bind it n times - after checking that both give the same value.
 
 Workloads: field tables at 2^20, 2^22, 2^24 in batches of 1 and 8; u8, u64 and i128 columns of 2^24 entries from host
-memory and from device memory; one-hot evaluation and pushforward at T = 2^24 with K = 16, 256 (u8) and 2^16 (u16).
+memory and from device memory; one-hot evaluation and pushforward at T = 2^24 with K = 16, 256 (u8), 2^16 (u16) and
+2^20, 2^24 (u32: RAM-sized address spaces, checked against the device evaluation of the pushforward table).
 Reports per workload the call's device time (CUDA events on the session's stream around the whole call: eq tables,
 kernel, lanes; median of 10 after a warm-up), the clone + bind route's device time, and the call against its bound:
 the larger of its table bytes over the data-sheet 3.35 TB/s HBM and its integer work over the Montgomery-product rate
@@ -11,7 +12,7 @@ measured in the same run (jb_diag_mul_throughput; an unreduced 256 x 256 product
 product, a 256 x 32w one as w/16). Reads the card's name and power limit in the same run.
 Output: one JSON line per workload on stdout, and in FILE with --out.
 
-usage: python tools/eval_bench.py [--out FILE] [--quick]"""
+usage: python tools/eval_bench.py [--out FILE] [--quick] [--one-hot-only]"""
 import argparse
 import ctypes
 import json
@@ -69,6 +70,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--quick", action="store_true", help="small sizes only (a rehearsal of the script)")
+    ap.add_argument("--one-hot-only", action="store_true", help="the one-hot workloads only")
     a = ap.parse_args()
     name, power = card()
     s = jolt_b200.Session(0, cuda_stream=torch.cuda.current_stream().cuda_stream)
@@ -90,7 +92,7 @@ def main():
     big = sizes[-1]
     pt_all = O.random_fr(1, 48)
     # ---- field tables
-    for n in sizes:
+    for n in ([] if a.one_hot_only else sizes):
         for batch in (1, 8):
             keep = [random_table(n, 10 * n + b) for b in range(batch)]
             polys = [Polynomial.wrap_device(s, t.data_ptr(), 1 << n) for t in keep]
@@ -119,7 +121,7 @@ def main():
     # ---- compact columns
     rng = np.random.Generator(np.random.PCG64(5))
     pt = pt_all[:big]
-    for kind, words in (("u8", 1), ("u64", 2), ("i128", 4)):
+    for kind, words in (() if a.one_hot_only else (("u8", 1), ("u64", 2), ("i128", 4))):
         if kind == "u8":
             col = rng.integers(0, 256, size=1 << big, dtype=np.uint8)
         elif kind == "u64":
@@ -181,6 +183,28 @@ def main():
                 g.free()
         ms = device_ms(pf)
         emit(dict(workload="one_hot_pushforward", K=K, log_t=big), T * col.itemsize, T, ms)
+    # ---- one-hot, u32 columns (the none value 0xFFFFFFFF is never drawn below K <= 2^24)
+    for K in ((1 << 8, 1 << 10) if a.quick else (1 << 20, 1 << 24)):
+        col = rng.integers(0, K, size=T).astype(np.uint32)
+        dcol = torch.from_numpy(col.view(np.int32)).cuda()
+        lk = K.bit_length() - 1
+        ptk = pt_all[:big + lk]
+        got = one_hot_evaluate(s, dcol, K, ptk)[0]
+        G = one_hot_pushforward(s, dcol, K, ptk[:big])[0]
+        assert got == Polynomial.batch_evaluate([G], ptk[big:])[0]
+        G.free()
+        ms = device_ms(lambda: one_hot_evaluate(s, dcol, K, ptk))
+        # the K-entry eq table is built and gathered (through L2) as well as the column read
+        emit(dict(workload="one_hot_evaluate", K=K, log_t=big, kind="u32"), T * 4 + 32 * K, T / 2, ms)
+
+        def pf():
+            for g in one_hot_pushforward(s, dcol, K, ptk[:big]):
+                g.free()
+        ms = device_ms(pf)
+        # bins: K x 64 B of lanes zeroed, read and converted into a K-entry table
+        emit(dict(workload="one_hot_pushforward", K=K, log_t=big, kind="u32"), T * 4 + 64 * K * 2 + 32 * K, T, ms)
+        del dcol
+        torch.cuda.empty_cache()
     if a.out:
         pathlib.Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         pathlib.Path(a.out).write_text("\n".join(lines) + "\n")

@@ -3,7 +3,8 @@
 Workloads:
   - registers-shaped: K = 128, A = 3 (rs1, rs2 reads, rd write, each its own u8 column, 10 % none), T = 2^20, 2^22, 2^24;
   - RAM-shaped: K = 2^16, one u16 column read (c = 1, d = 0) and written (c = gamma, d = 1), 5 % none cycles, T = 2^22,
-    with uniform addresses and with a local stream (a random walk of step -2..2).
+    with uniform addresses and with a local stream (a random walk of step -2..2);
+  - RAM at a real address space: K = 2^22, one u32 column (none = 0xFFFFFFFF), otherwise as above, T = 2^22.
 Values are u64 columns, inc an i64 column (0 where the write is none), init u64. The member does not check the value
 precondition and the rounds' cost does not depend on it, so the values are random. Reports per workload:
   - ms: host wall time of creation + every round + final evaluations (final_evals waits for the device); median of 3
@@ -17,7 +18,7 @@ eq table, 6 x 2^27 entries) proving the same rounds, tables already on the devic
 evaluations, median of 2 after 1 warm-up) next to the member's rw_ms on the same columns; both agree round by round.
 Reads the card's name, power limit, maximum and current SM clock in the same run. One JSON line per workload on stdout, and in FILE with --out.
 
-usage: python tools/rw_bench.py [--out FILE] [--quick]"""
+usage: python tools/rw_bench.py [--out FILE] [--quick] [--only PREFIX]"""
 import argparse
 import json
 import pathlib
@@ -49,13 +50,17 @@ def sm_clocks():
         return [f"unknown ({e})", "unknown"]
 
 
+def none_of(K):
+    return 0xFF if K <= 256 else 0xFFFF if K <= (1 << 16) else 0xFFFFFFFF
+
+
 def columns(rng, K, T, n, none_frac, local):
-    none = 0xFF if K <= 256 else 0xFFFF
+    none = none_of(K)
     hi = min(K, none)
     out = []
     for _ in range(n):
         a = (np.cumsum(rng.integers(-2, 3, T)) % hi) if local else rng.integers(0, hi, T)
-        a = a.astype(np.uint8 if K <= 256 else np.uint16)
+        a = a.astype(np.uint8 if K <= 256 else np.uint16 if K <= (1 << 16) else np.uint32)
         a[rng.random(T) < none_frac] = none
         out.append(a)
     return out
@@ -63,7 +68,7 @@ def columns(rng, K, T, n, none_frac, local):
 
 def live_entries(cols, K, T):
     """Distinct (row, address) pairs after each of the log2 T cycle binds, starting from the unbound matrix."""
-    none = 0xFF if K <= 256 else 0xFFFF
+    none = none_of(K)
     j = np.arange(T, dtype=np.int64)
     x = np.concatenate([j[c != none] * K + c[c != none].astype(np.int64) for c in cols])
     x = np.unique(x)
@@ -78,10 +83,10 @@ def live_entries(cols, K, T):
 def run(sess, wl, reps):
     K, T, cols, acc_spec, write = wl["K"], wl["T"], wl["cols"], wl["acc"], wl["write"]
     rng = np.random.default_rng(1)
-    dev_cols = [torch.from_numpy(c.view(np.uint8) if c.dtype == np.uint8 else c.view(np.int16)).cuda() for c in cols]
+    dev_cols = [torch.from_numpy(c.view({1: np.uint8, 2: np.int16, 4: np.int32}[c.itemsize])).cuda() for c in cols]
     vals = [torch.from_numpy(rng.integers(0, 1 << 62, T).astype(np.int64)).cuda() for _ in acc_spec]
     wcol = cols[acc_spec[write][0]]
-    none = 0xFF if K <= 256 else 0xFFFF
+    none = none_of(K)
     inc = rng.integers(-(1 << 40), 1 << 40, T).astype(np.int64)
     inc[wcol == none] = 0
     inc_t = torch.from_numpy(inc).cuda()
@@ -169,6 +174,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out")
     ap.add_argument("--quick", action="store_true", help="T = 2^16 only (a rehearsal)")
+    ap.add_argument("--only", default=None, help="only the workloads whose name starts with this (no dense route)")
     args = ap.parse_args()
     rng = np.random.default_rng(0)
     name, power = card()
@@ -183,6 +189,13 @@ def main():
         T = 1 << logt
         wls.append(dict(name=f"ram_{'local' if local else 'uniform'}_T2^{logt}", K=1 << 16, T=T,
                         cols=columns(rng, 1 << 16, T, 1, 0.05, local), acc=[(0, 0), (0, 1)], write=1))
+    for local in (False, True):
+        logt, logk = (16, 18) if args.quick else (22, 22)
+        T = 1 << logt
+        wls.append(dict(name=f"ram_u32_K2^{logk}_{'local' if local else 'uniform'}_T2^{logt}", K=1 << logk, T=T,
+                        cols=columns(rng, 1 << logk, T, 1, 0.05, local), acc=[(0, 0), (0, 1)], write=1))
+    if args.only:
+        wls = [wl for wl in wls if wl["name"].startswith(args.only)]
     lines = []
     for wl in wls:
         A = len(wl["acc"])
@@ -197,7 +210,7 @@ def main():
                    sm_clock_max=sm_max, sm_clock_after=sm_now)
         print(json.dumps(rec), flush=True)
         lines.append(json.dumps(rec))
-    if not args.quick:
+    if not args.quick and not args.only:
         rec = dense_comparison(sess, 2)
         rec.update(card=name, power_limit=power, sm_clock_max=sm_clocks()[0])
         print(json.dumps(rec), flush=True)
