@@ -223,7 +223,6 @@ void jb_ctx_destroy(jb_ctx* c) {
         if (kv.second.pre_small) cudaFreeAsync(kv.second.pre_small, c->stream);
     }
     c->srs.clear();
-    c->msm_release();
     if (c->d_partial) cudaFreeAsync(c->d_partial, c->stream);
     if (c->d_small) cudaFree(c->d_small);
     if (c->h_small) cudaFreeHost(c->h_small);

@@ -194,7 +194,6 @@ struct jb_ctx {
         if (t.alt && t.alt_owned) dev_free(t.alt);
         t.buf = t.alt = nullptr;
     }
-    void msm_release();
 };
 
 // Blocks of `block` threads for a grid-stride pass over `items`: one per `block` items, at most one wave of

@@ -221,31 +221,12 @@ def test_small_msm_over_precomputed_srs(sess, srs_bases, n):
     assert g1_jacobian_to_affine(bases.msm(sc, offset=off)) == want2
 
 
-@pytest.fixture
-def force_affine_levels():
-    """The batched-affine levels (msm_affine.cuh) normally serve only windows x terms >= 2^26; JB_MSM_BA_MIN_LOG = 0
-    sends every field-scalar MSM that does not fit the small table through them (the library reads it per call)."""
-    import os
-    old = {k: os.environ.get(k) for k in ("JB_MSM_BA", "JB_MSM_BA_MIN_LOG")}
-    os.environ["JB_MSM_BA_MIN_LOG"] = "0"
-
-    def set_levels(levels: int):
-        os.environ["JB_MSM_BA"] = str(levels)
-    yield set_levels
-    for k, v in old.items():
-        if v is None:
-            os.environ.pop(k, None)
-        else:
-            os.environ[k] = v
-
-
-@pytest.mark.parametrize("levels", [1, 2, 3, 5])
-def test_msm_batched_affine_levels_match_oracle(sess, srs_bases, force_affine_levels, levels):
-    """Same group value with the first `levels` halvings of every bucket done by batched affine additions
-    (the device form of crates/jolt-crypto/src/ec/bn254/batch_addition.rs:53-150, made complete)."""
-    force_affine_levels(levels)
+@pytest.mark.parametrize("seed", [0xBB, 0xBC, 0xBD, 0xBF])
+def test_msm_odd_length_and_window10_table_match_oracle(sess, srs_bases, seed):
+    """2^13 and 2^13 - 37 terms, over plain bases (one bucket set per window) and over a window-10 shared table (one
+    bucket set for all windows): same group value as the oracle's Pippenger."""
     for n in (1 << 13, (1 << 13) - 37):
-        sc = rand_limbs(0xBA + levels, n)
+        sc = rand_limbs(seed, n)
         want = oracle_affine(*C.g1_msm_pippenger(srs_bases[:n], sc, 0, C.max_threads()))
         plain = G1Bases.from_affine(sess, srs_bases[:n])
         assert g1_jacobian_to_affine(plain.msm(sc)) == want
@@ -255,10 +236,10 @@ def test_msm_batched_affine_levels_match_oracle(sess, srs_bases, force_affine_le
         pre.free()
 
 
-def test_msm_batched_affine_exceptional_pairs(sess, force_affine_levels):
-    """What the reference's batch addition excludes by precondition and an MSM cannot: equal points in a pair (tangent),
-    opposite points (identity result, then an identity operand one level up), identity bases, all terms in one bucket."""
-    force_affine_levels(4)
+def test_msm_crowded_buckets_and_cancelling_terms(sess):
+    """Inputs that crowd the buckets or cancel inside them: every term in one bucket (the XYZZ walk doubles when it adds
+    a point to itself), P and -P alternating (a bucket sum that returns to the identity, and the identity as an
+    operand afterwards), identity bases, repeated points whose pair sums coincide."""
     n = 1 << 13
     # every base the same point, every scalar the same: each bucket is a list of n copies of one point
     one = [O.g1_scalar_mul(O.G1_GEN, 9)] * n
@@ -285,7 +266,6 @@ def test_msm_batched_affine_exceptional_pairs(sess, force_affine_levels):
     got = g1_jacobian_to_affine(jolt_b200.msm(sess, g1_affine_limbs(bases), C.ints_to_mont(svals)))
     assert got == O.g1_scalar_mul(O.G1_GEN, total)
     # closed form over (i + 1) G with uniform scalars at 2^16, plain and precomputed
-    force_affine_levels(3)
     n = 1 << 16
     gen = G1Bases.generate_multiples(sess, G, n)
     sc = rand_limbs(0x5CA1A2, n)
