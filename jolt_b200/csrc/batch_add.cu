@@ -155,9 +155,9 @@ extern "C" int jb_g1_batch_add(jb_ctx* c, jb_srs bases, const uint64_t* set_offs
     if (!c || (nsets && (!set_offsets || !out_xy))) return JB_ERR_INVALID;
     if (nsets == 0) return JB_OK;
     Guard g(c);
-    auto it = c->srs.find(bases);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    const Srs& srs = it->second;
+    Srs* found = nullptr;
+    if (const int st = c->find_srs(bases, &found)) return st;
+    const Srs& srs = *found;
     const size_t total = set_offsets[nsets];
     if (total >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "batch_add: fewer than 2^31 indices per call");
     if (total && !indices) return JB_ERR_INVALID;
@@ -172,14 +172,15 @@ extern "C" int jb_g1_batch_add(jb_ctx* c, jb_srs bases, const uint64_t* set_offs
         cnt[s] = set_offsets[s + 1] - set_offsets[s];
         max_cnt = cnt[s] > max_cnt ? cnt[s] : max_cnt;
     }
+    Scratch scratch(c);
     uint32_t* d_idx = nullptr;
     uint64_t *d_w[2] = {nullptr, nullptr}, *d_off = nullptr;
     int st = JB_OK;
     const size_t w_elems = total / 2 + nsets + 1;  // level-1 size bound: sum ceil(cnt / 2)
-    if (total) st = c->dev_alloc((void**)&d_idx, total * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_w[0], w_elems * 64);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_w[1], w_elems * 64);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_off, 3 * (nsets + 1) * 8);
+    if (total) st = scratch.alloc(total * 4, &d_idx);
+    if (st == JB_OK) st = scratch.alloc(w_elems * 64, &d_w[0]);
+    if (st == JB_OK) st = scratch.alloc(w_elems * 64, &d_w[1]);
+    if (st == JB_OK) st = scratch.alloc(3 * (nsets + 1) * 8, &d_off);
     if (st == JB_OK && total)
         st = c->check(cudaMemcpyAsync(d_idx, indices, total * 4, cudaMemcpyHostToDevice, c->stream), "batch_add indices H2D");
     std::vector<uint64_t> offs(3 * (nsets + 1));
@@ -257,9 +258,5 @@ extern "C" int jb_g1_batch_add(jb_ctx* c, jb_srs bases, const uint64_t* set_offs
         }
         if (st == JB_OK && from_bases) st = c->check(cudaStreamSynchronize(c->stream), "batch_add sync");
     }
-    if (d_idx) c->dev_free(d_idx);
-    if (d_w[0]) c->dev_free(d_w[0]);
-    if (d_w[1]) c->dev_free(d_w[1]);
-    if (d_off) c->dev_free(d_off);
     return st;
 }

@@ -78,9 +78,10 @@ int jbi::eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* sc
     // n > 11: prefix table over the leading n-11 variables (recursively), the block-independent table
     // over the trailing 8, and one streaming pass that writes every output exactly once.
     size_t hi_vars = nvars - EQ_BLOCK_VARS;
+    Scratch scratch(c);
     uint64_t *d_prefix = nullptr, *d_low8 = nullptr;
-    int st = c->dev_alloc((void**)&d_prefix, ((size_t)1 << hi_vars) * 32);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_low8, 256 * 32);
+    int st = scratch.alloc(((size_t)1 << hi_vars) * 32, &d_prefix);
+    if (st == JB_OK) st = scratch.alloc(256 * 32, &d_low8);
     if (st == JB_OK) st = eq_build(c, r, hi_vars, scale, d_prefix);
     // the block's first 3 variables are expanded in registers (a warp's store covers 1 KiB), its last 8 come from low8
     if (st == JB_OK) st = eq_build(c, r + 4 * (hi_vars + 3), 8, nullptr, d_low8);
@@ -103,8 +104,6 @@ int jbi::eq_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* sc
         c->launches++;
         st = c->check(cudaGetLastError(), "eq_stream_kernel launch");
     }
-    if (d_prefix) c->dev_free(d_prefix);
-    if (d_low8) c->dev_free(d_low8);
     return st;
 }
 
@@ -217,11 +216,7 @@ void jb_ctx_destroy(jb_ctx* c) {
         if (r.d_state) cudaFree(r.d_state);
     }
     c->tail_pool.clear();
-    for (auto& kv : c->srs) {
-        if (kv.second.xy) cudaFreeAsync(kv.second.xy, c->stream);
-        if (kv.second.pre) cudaFreeAsync(kv.second.pre, c->stream);
-        if (kv.second.pre_small) cudaFreeAsync(kv.second.pre_small, c->stream);
-    }
+    for (auto& kv : c->srs) c->release(kv.second);
     c->srs.clear();
     if (c->d_partial) cudaFreeAsync(c->d_partial, c->stream);
     if (c->d_small) cudaFree(c->d_small);
@@ -303,30 +298,29 @@ int jb_ctx_timing_collect(jb_ctx* c, int* kinds, uint64_t* items, int* ms_m, dou
 }
 
 // ---- tables ------------------------------------------------------------------------------
+// A table of len entries for the call to fill and hand over (context lock held).
+static int new_table(jb_ctx* c, size_t len, Table& t) {
+    t.cap = t.len = len;
+    return c->dev_alloc((void**)&t.buf, len * 32);
+}
+
 int jb_table_alloc(jb_ctx* c, size_t len, jb_table* out) {
     if (!c || !out || len == 0) return JB_ERR_INVALID;
     Guard g(c);
     Table t;
-    int st = c->dev_alloc((void**)&t.buf, len * 32);
-    if (st != JB_OK) return st;
-    t.cap = t.len = len;
-    t.buf_owned = true;
-    *out = c->next_id++;
-    c->tables[*out] = t;
-    return JB_OK;
+    return c->hand_over(new_table(c, len, t), t, out);
 }
 
 int jb_table_upload(jb_ctx* c, const uint64_t* limbs, size_t len, jb_table* out) {
-    if (!c || !limbs) return JB_ERR_INVALID;
-    int st = jb_table_alloc(c, len, out);
-    if (st != JB_OK) return st;
+    if (!c || !limbs || !out || len == 0) return JB_ERR_INVALID;
     Guard g(c);
-    Table& t = c->tables[*out];
-    st = c->check(cudaMemcpyAsync(t.buf, limbs, len * 32, cudaMemcpyHostToDevice, c->stream), "table upload");
+    Table t;
+    int st = new_table(c, len, t);
+    if (st == JB_OK) st = c->check(cudaMemcpyAsync(t.buf, limbs, len * 32, cudaMemcpyHostToDevice, c->stream), "table upload");
     // the host buffer is borrowed for the duration of the call only: with pinned / registered memory the copy is
     // truly asynchronous, so wait for it (pageable memory is staged before cudaMemcpyAsync returns anyway)
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "table upload sync");
-    return st;
+    return c->hand_over(st, t, out);
 }
 
 int jb_table_wrap_device(jb_ctx* c, void* dptr, size_t len, jb_table* out) {
@@ -336,9 +330,7 @@ int jb_table_wrap_device(jb_ctx* c, void* dptr, size_t len, jb_table* out) {
     t.buf = (uint64_t*)dptr;
     t.cap = t.len = len;
     t.buf_owned = false;
-    *out = c->next_id++;
-    c->tables[*out] = t;
-    return JB_OK;
+    return c->hand_over(JB_OK, t, out);
 }
 
 int jb_table_len(jb_ctx* c, jb_table h, size_t* len) {
@@ -372,18 +364,14 @@ int jb_table_download(jb_ctx* c, jb_table h, uint64_t* out, size_t len) {
 
 int jb_table_clone(jb_ctx* c, jb_table h, jb_table* out) {
     if (!c || !out) return JB_ERR_INVALID;
-    size_t len;
-    {
-        Guard g(c);
-        Table* t = c->find(h);
-        if (!t) return c->fail(JB_ERR_INVALID, "unknown table handle");
-        len = t->len;
-    }
-    int st = jb_table_alloc(c, len, out);
-    if (st != JB_OK) return st;
     Guard g(c);
-    return c->check(cudaMemcpyAsync(c->tables[*out].buf, c->tables[h].buf, len * 32, cudaMemcpyDeviceToDevice, c->stream),
-                    "table clone");
+    const Table* src = c->find(h);
+    if (!src) return c->fail(JB_ERR_INVALID, "unknown table handle");
+    Table t;
+    int st = new_table(c, src->len, t);
+    if (st == JB_OK)
+        st = c->check(cudaMemcpyAsync(t.buf, src->buf, src->len * 32, cudaMemcpyDeviceToDevice, c->stream), "table clone");
+    return c->hand_over(st, t, out);
 }
 
 int jb_table_free(jb_ctx* c, jb_table h) {
@@ -410,10 +398,11 @@ int jb_eq_evals(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scal
     for (size_t i = 0; i < nvars; ++i)
         if (!canonical_fr(r + 4 * i)) return c->fail(JB_ERR_INVALID, "eq: point limbs not canonical");
     if (scale && !canonical_fr(scale)) return c->fail(JB_ERR_INVALID, "eq: scale limbs not canonical");
-    int st = jb_table_alloc(c, (size_t)1 << nvars, out);
-    if (st != JB_OK) return st;
     Guard g(c);
-    return eq_build(c, r, nvars, scale, c->tables[*out].buf);
+    Table t;
+    int st = new_table(c, (size_t)1 << nvars, t);
+    if (st == JB_OK) st = eq_build(c, r, nvars, scale, t.buf);
+    return c->hand_over(st, t, out);
 }
 
 int jb_eq_evals_aligned_block(jb_ctx* c, const uint64_t* r, size_t nvars, size_t start_index, size_t block_size,
@@ -443,10 +432,11 @@ int jb_vec_op(jb_ctx* c, int field, int op, const uint64_t* a, const uint64_t* b
     if (!c || !a || !b || !out || op < 0 || op > 5 || (field != 0 && field != 1)) return JB_ERR_INVALID;
     if (n == 0) return JB_OK;
     Guard g(c);
+    Scratch scratch(c);
     uint64_t *da = nullptr, *db = nullptr, *dd = nullptr;
-    int st = c->dev_alloc((void**)&da, n * 32);
-    if (st == JB_OK) st = c->dev_alloc((void**)&db, n * 32);
-    if (st == JB_OK) st = c->dev_alloc((void**)&dd, n * 32);
+    int st = scratch.alloc(n * 32, &da);
+    if (st == JB_OK) st = scratch.alloc(n * 32, &db);
+    if (st == JB_OK) st = scratch.alloc(n * 32, &dd);
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, c->stream), "vec H2D");
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(db, b, n * 32, cudaMemcpyHostToDevice, c->stream), "vec H2D");
     if (st == JB_OK) {
@@ -458,9 +448,6 @@ int jb_vec_op(jb_ctx* c, int field, int op, const uint64_t* a, const uint64_t* b
     }
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(out, dd, n * 32, cudaMemcpyDeviceToHost, c->stream), "vec D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "vec sync");
-    if (da) c->dev_free(da);
-    if (db) c->dev_free(db);
-    if (dd) c->dev_free(dd);
     return st;
 }
 
@@ -493,9 +480,10 @@ __global__ void __launch_bounds__(256) mul_chain_kernel(uint64_t* io, int iters)
 extern "C" int jb_diag_mul_throughput(jb_ctx* c, int field, int variant, int iters, int blocks, double* out_gops) {
     if (!c || !out_gops || iters < 1 || blocks < 1 || variant < 0 || variant > 2) return JB_ERR_INVALID;
     Guard g(c);
+    Scratch scratch(c);
     size_t threads = (size_t)blocks * 256;
     uint64_t* d = nullptr;
-    int st = c->dev_alloc((void**)&d, threads * 4 * 32);
+    int st = scratch.alloc(threads * 4 * 32, &d);
     if (st != JB_OK) return st;
     std::vector<uint64_t> h(threads * 16);
     uint64_t sm = 0x1234;
@@ -521,7 +509,6 @@ extern "C" int jb_diag_mul_throughput(jb_ctx* c, int field, int variant, int ite
     }
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
-    c->dev_free(d);
     if (st == JB_OK) *out_gops = (double)threads * 2.0 * iters / (best * 1e-3) / 1e9;
     return st;
 }

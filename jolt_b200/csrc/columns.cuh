@@ -14,7 +14,6 @@
 #pragma once
 #include <algorithm>
 #include <string>
-#include <vector>
 
 #include "ctx.hpp"
 #include "small_scalar.cuh"
@@ -100,26 +99,19 @@ inline int copy_column(jb_ctx* c, const void* values, size_t bytes, int on_devic
                     "column copy");
 }
 
-// Columns of a call that reads them in place: host columns are copied to device memory allocated for the call and
-// freed with it; device columns are used as they are.
-struct Columns {
-    jb_ctx* c;
-    std::vector<void*> owned;
-    explicit Columns(jb_ctx* ctx) : c(ctx) {}
-    ~Columns() {
-        for (void* p : owned) c->dev_free(p);
+// A column a call reads in place: a host column is copied to device memory owned by the call's scratch, a device
+// column is used as it is.
+inline int get_column(Scratch& scratch, const void* src, size_t bytes, int on_device, const void** dst) {
+    if (on_device) {
+        *dst = src;
+        return JB_OK;
     }
-    int get(const void* src, size_t bytes, int on_device, const void** dst) {
-        if (on_device) {
-            *dst = src;
-            return JB_OK;
-        }
-        void* d = nullptr;
-        const int st = copy_column(c, src, bytes, 0, &d);
-        if (d) owned.push_back(d);
-        *dst = d;
-        return st;
-    }
-};
+    void* d = nullptr;
+    int st = scratch.alloc(bytes, &d);
+    if (st == JB_OK)
+        st = scratch.c->check(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, scratch.c->stream), "column copy");
+    *dst = d;
+    return st;
+}
 
 }  // namespace jb

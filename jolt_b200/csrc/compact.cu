@@ -75,13 +75,13 @@ extern "C" {
 int jb_table_upload_small(jb_ctx* c, const void* values, size_t len, int kind, jb_table* out) {
     if (!c || !values || !out || len == 0) return JB_ERR_INVALID;
     if (!compact_kind(kind)) return c->fail(JB_ERR_INVALID, "upload_small: unknown scalar kind");
-    int st = jb_table_alloc(c, len, out);
-    if (st != JB_OK) return st;
     Guard g(c);
-    Table& t = c->tables[*out];
-    Columns cols(c);
+    Scratch scratch(c);
+    Table t;
+    t.cap = t.len = len;
+    int st = c->dev_alloc((void**)&t.buf, len * 32);
     const void* d_vals = nullptr;
-    st = cols.get(values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
+    if (st == JB_OK) st = get_column(scratch, values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
     // (the caller's buffer is only borrowed for the call: a pinned source makes the copy truly asynchronous)
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "upload_small sync");
     if (st == JB_OK) {
@@ -89,11 +89,7 @@ int jb_table_upload_small(jb_ctx* c, const void* values, size_t len, int kind, j
         c->launches++;
         st = c->check(cudaGetLastError(), "promote_small_kernel launch");
     }
-    if (st != JB_OK) {
-        c->release(t);
-        c->tables.erase(*out);
-    }
-    return st;
+    return c->hand_over(st, t, out);
 }
 
 int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, const uint64_t r[4], int order, jb_table* out) {
@@ -103,10 +99,11 @@ int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, con
     if (HostFr::geq_p(r)) return c->fail(JB_ERR_INVALID, "bind_small: challenge limbs not canonical (>= r)");
     if (order != JB_HIGH_TO_LOW && order != JB_LOW_TO_HIGH) return c->fail(JB_ERR_INVALID, "bind_small: unknown binding order");
     const size_t half = len / 2;
-    int st = jb_table_alloc(c, half, out);
-    if (st != JB_OK) return st;
     Guard g(c);
-    Table& t = c->tables[*out];
+    Scratch scratch(c);
+    Table t;
+    t.cap = t.len = half;
+    int st = c->dev_alloc((void**)&t.buf, half * 32);
     const HostFr r2{{HostFr::R2[0], HostFr::R2[1], HostFr::R2[2], HostFr::R2[3]}};
     const HostFr sr = HostFr::from_limbs(r) * r2;
     BindScalar s;
@@ -114,9 +111,8 @@ int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, con
         s.w[2 * i] = (uint32_t)sr.l[i];
         s.w[2 * i + 1] = (uint32_t)(sr.l[i] >> 32);
     }
-    Columns cols(c);
     const void* d_vals = nullptr;
-    st = cols.get(values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
+    if (st == JB_OK) st = get_column(scratch, values, len * (size_t)small_kind_bytes(kind), 0, &d_vals);
     // (the caller's buffer is only borrowed for the call: a pinned source makes the copy truly asynchronous)
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "bind_small sync");
     if (st == JB_OK) {
@@ -127,11 +123,7 @@ int jb_table_bind_small(jb_ctx* c, const void* values, size_t len, int kind, con
         c->launches++;
         st = c->check(cudaGetLastError(), "bind_small_kernel launch");
     }
-    if (st != JB_OK) {
-        c->release(t);
-        c->tables.erase(*out);
-    }
-    return st;
+    return c->hand_over(st, t, out);
 }
 
 }  // extern "C"

@@ -42,7 +42,6 @@ struct Srs {
     size_t pre_small_len = 0;
 };
 
-struct MsmWorkspace;  // msm.cu
 struct ResidentRun;   // resident.cu: one launched resident_rounds_kernel and the members it serves
 
 // Host-mapped mailbox + device state + private stream + event for one resident kernel; pooled per context so
@@ -105,7 +104,6 @@ struct jb_ctx {
     uint64_t* d_result_alias = nullptr;  // device address of h_result
     unsigned int* d_counter = nullptr;   // last-block ticket counter (zero between launches)
     uint64_t result_seq = 0;
-    MsmWorkspace* msm = nullptr;
     // multi-GPU (comm.cu): NCCL communicator + the lanes buffer the per-round all-reduce runs on
     void* nccl_comm = nullptr;
     int world = 1, rank = 0;
@@ -193,6 +191,63 @@ struct jb_ctx {
         if (t.buf && t.buf_owned) dev_free(t.buf);
         if (t.alt && t.alt_owned) dev_free(t.alt);
         t.buf = t.alt = nullptr;
+    }
+    void release(Srs& s) {
+        dev_free(s.xy);
+        dev_free(s.pre);
+        dev_free(s.pre_small);
+        s.xy = s.pre = s.pre_small = nullptr;
+    }
+    // Hands a table a call has built to the caller: on success it is registered under a new handle (*out), on
+    // failure (st != JB_OK) its buffers are released.
+    int hand_over(int st, Table& t, jb_table* out) {
+        if (st != JB_OK) {
+            release(t);
+            return st;
+        }
+        *out = next_id++;
+        tables[*out] = t;
+        return JB_OK;
+    }
+    int hand_over(int st, Srs& s, jb_srs* out) {
+        if (st != JB_OK) {
+            release(s);
+            return st;
+        }
+        *out = next_id++;
+        srs[*out] = s;
+        return JB_OK;
+    }
+    // *out = the SRS of handle h, or the failure every entry point reports for an unknown handle.
+    int find_srs(jb_srs h, Srs** out) {
+        auto it = srs.find(h);
+        if (it == srs.end()) return fail(JB_ERR_INVALID, "unknown srs handle");
+        *out = &it->second;
+        return JB_OK;
+    }
+};
+
+// The device memory one call allocates for itself: every buffer alloc() hands out is freed, stream-ordered on the
+// context's stream, by release() or when the scratch goes out of scope. The frees must run under the context lock:
+// declare the scratch after the call's CtxGuard, in the same scope.
+struct Scratch {
+    jb_ctx* c;
+    std::vector<void*> owned;
+    explicit Scratch(jb_ctx* ctx) : c(ctx) {}
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { release(); }
+    template <class T>
+    int alloc(size_t bytes, T** p) {
+        void* d = nullptr;
+        const int st = c->dev_alloc(&d, bytes);
+        if (d) owned.push_back(d);
+        *p = static_cast<T*>(d);
+        return st;
+    }
+    void release() {
+        for (void* p : owned) c->dev_free(p);
+        owned.clear();
     }
 };
 

@@ -278,14 +278,16 @@ int jb_hyperkzg_open(jb_ctx* c, jb_srs srs, jb_table evals, const uint64_t* poin
         Table* t = c->find(evals);
         if (!t) return c->fail(JB_ERR_INVALID, "unknown table handle");
         if (t->len != n) return c->fail(JB_ERR_INVALID, "hyperkzg: evaluation count must be 2^ell");
-        auto it = c->srs.find(srs);
-        if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-        if (it->second.n < n) return c->fail(JB_ERR_LENGTH, "HyperKZGError::SrsTooSmall");
+        Srs* s = nullptr;
+        if (const int st = c->find_srs(srs, &s)) return st;
+        if (s->n < n) return c->fail(JB_ERR_LENGTH, "HyperKZGError::SrsTooSmall");
         for (size_t i = 0; i < ell; ++i)
             if (HostFr::geq_p(point + 4 * i)) return c->fail(JB_ERR_INVALID, "hyperkzg: point limbs not canonical");
         d_evals = t->buf;
     }
-    // ---- workspace -------------------------------------------------------------------------------
+    // ---- workspace: the phases take the context lock one at a time (the MSMs take it themselves), so the scratch is
+    // released explicitly, under the lock, in the last phase ---------------------------------------------
+    Scratch scratch(c);
     uint64_t *d_folded = nullptr, *d_b = nullptr, *d_h = nullptr, *d_tt = nullptr, *d_bt = nullptr, *d_bs = nullptr,
              *d_vals = nullptr;
     const int Lb = chunk_for(n);
@@ -294,13 +296,13 @@ int jb_hyperkzg_open(jb_ctx* c, jb_srs srs, jb_table evals, const uint64_t* poin
     int st;
     {
         Guard g(c);
-        st = c->dev_alloc((void**)&d_folded, n * 32);  // sum_{j>=1} 2^(ell-j) < n
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_b, n * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_h, (size_t)HZ_POINTS * n * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_tt, nblocks_b * HZ_THREADS * HZ_POINTS * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_bt, 1024 * HZ_POINTS * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_bs, 1024 * HZ_POINTS * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_vals, (ell + 1) * HZ_POINTS * 32);
+        st = scratch.alloc(n * 32, &d_folded);  // sum_{j>=1} 2^(ell-j) < n
+        if (st == JB_OK) st = scratch.alloc(n * 32, &d_b);
+        if (st == JB_OK) st = scratch.alloc((size_t)HZ_POINTS * n * 32, &d_h);
+        if (st == JB_OK) st = scratch.alloc(nblocks_b * HZ_THREADS * HZ_POINTS * 32, &d_tt);
+        if (st == JB_OK) st = scratch.alloc(1024 * HZ_POINTS * 32, &d_bt);
+        if (st == JB_OK) st = scratch.alloc(1024 * HZ_POINTS * 32, &d_bs);
+        if (st == JB_OK) st = scratch.alloc((ell + 1) * HZ_POINTS * 32, &d_vals);
         // ---- phase 1: fold (scheme.rs:88-114): P_i = bind_low_to_high(P_(i-1), point[ell - i]) ------------
         const uint64_t* prev = d_evals;
         size_t off = 0, len = n;
@@ -400,13 +402,7 @@ int jb_hyperkzg_open(jb_ctx* c, jb_srs srs, jb_table evals, const uint64_t* poin
     }
     {
         Guard g(c);
-        c->dev_free(d_folded);
-        c->dev_free(d_b);
-        c->dev_free(d_h);
-        c->dev_free(d_tt);
-        c->dev_free(d_bt);
-        c->dev_free(d_bs);
-        c->dev_free(d_vals);
+        scratch.release();
     }
     return st;
 }

@@ -86,14 +86,14 @@ int check_terms(jb_ctx* c, const jb_lc_term* terms, size_t count, size_t len, st
     return JB_OK;
 }
 
-// The column pointers of the checked descriptors: host columns are copied to the device for the call (owned by cols).
-int load_columns(Columns& cols, const jb_lc_term* terms, size_t count, std::vector<LcTerm>& desc) {
+// The column pointers of the checked descriptors: host columns are copied to the device for the call (owned by scratch).
+int load_columns(Scratch& scratch, const jb_lc_term* terms, size_t count, std::vector<LcTerm>& desc) {
     int st = JB_OK;
     for (size_t i = 0; i < count && st == JB_OK; ++i) {
         const jb_lc_term& in = terms[i];
         if (in.type == JB_LC_TABLE) continue;
         const size_t bytes = in.len * (size_t)small_kind_bytes(in.kind);
-        st = cols.get(in.values, bytes, in.on_device, &desc[i].ptr);
+        st = get_column(scratch, in.values, bytes, in.on_device, &desc[i].ptr);
     }
     return st;
 }

@@ -124,13 +124,13 @@ int jb_table_linear_combination(jb_ctx* c, const jb_lc_term* terms, size_t count
     std::vector<LcTerm> desc;
     int st = check_terms(c, terms, count, len, desc);
     if (st != JB_OK) return st;
-    Columns cols(c);
-    st = load_columns(cols, terms, count, desc);
+    Scratch scratch(c);
+    st = load_columns(scratch, terms, count, desc);
     LcTerm* d_terms = nullptr;
     unsigned int* d_bad = nullptr;
     Table t;
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_terms, count * sizeof(LcTerm));
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_bad, sizeof(unsigned int));
+    if (st == JB_OK) st = scratch.alloc(count * sizeof(LcTerm), &d_terms);
+    if (st == JB_OK) st = scratch.alloc(sizeof(unsigned int), &d_bad);
     if (st == JB_OK) st = c->dev_alloc((void**)&t.buf, len * 32);
     if (st == JB_OK)
         st = c->check(cudaMemcpyAsync(d_terms, desc.data(), count * sizeof(LcTerm), cudaMemcpyHostToDevice, c->stream),
@@ -145,16 +145,8 @@ int jb_table_linear_combination(jb_ctx* c, const jb_lc_term* terms, size_t count
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, c->stream), "linear_combination flag D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "linear_combination sync");
     if (st == JB_OK && bad) st = fail_bad_address(c);
-    c->dev_free(d_terms);
-    c->dev_free(d_bad);
-    if (st != JB_OK) {
-        c->dev_free(t.buf);
-        return st;
-    }
     t.cap = t.len = len;
-    *out = c->next_id++;
-    c->tables[*out] = t;
-    return JB_OK;
+    return c->hand_over(st, t, out);
 }
 
 }  // extern "C"

@@ -1036,8 +1036,9 @@ static int create_over_sources(jb_ctx* c, MemberKind kind, const jb_source* sour
         if (!mem) return JB_ERR_OOM;
         mem->tables.resize(nsources);
         mem->src.resize(nsources);
+        Scratch scratch(c);
         unsigned int* d_flag = nullptr;
-        st = c->dev_alloc((void**)&d_flag, sizeof(unsigned int));
+        st = scratch.alloc(sizeof(unsigned int), &d_flag);
         if (st == JB_OK) st = c->check(cudaMemsetAsync(d_flag, 0, sizeof(unsigned int), c->stream), "expr sources: flag memset");
         for (size_t i = 0; i < nsources && st == JB_OK; ++i) {
             const jb_source& sr = sources[i];
@@ -1061,7 +1062,6 @@ static int create_over_sources(jb_ctx* c, MemberKind kind, const jb_source* sour
         // (the caller's columns are borrowed for the call only)
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "expr sources: creation sync");
         if (st == JB_OK && flag) st = fail_bad_address(c);
-        c->dev_free(d_flag);
         if (st != JB_OK) {
             discard_sources(mem);
             return st;
@@ -1254,15 +1254,15 @@ static int gather_into_tail(jb_member* mem) {  // called with the context lock h
             // rank order == global order for contiguous blocks under LowToHigh binding
             st = c->comm_allgather(mem->tables[j].buf, t.buf, len * 4);
         } else {
+            Scratch scratch(c);
             uint64_t* tmp = nullptr;
-            st = c->dev_alloc((void**)&tmp, tail->len * 32);
+            st = scratch.alloc(tail->len * 32, &tmp);
             if (st == JB_OK) st = c->comm_allgather(mem->tables[j].buf, tmp, len * 4);
             if (st == JB_OK) {
                 interleave_shards_kernel<<<(unsigned)((tail->len + 255) / 256), 256, 0, c->stream>>>(tmp, t.buf, len, G);
                 c->launches++;
                 st = c->check(cudaGetLastError(), "interleave_shards launch");
             }
-            c->dev_free(tmp);
         }
     }
     if (st != JB_OK) {

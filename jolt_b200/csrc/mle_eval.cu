@@ -192,9 +192,11 @@ int check_point(jb_ctx* c, const uint64_t* point, size_t nvars, const char* what
     return JB_OK;
 }
 
-// What every evaluation shares: the split of the point, its two eq tables, the launch shape and the lane tail.
+// What every evaluation shares: the split of the point, its two eq tables, the launch shape and the lane tail. Its
+// scratch owns these buffers and whatever else the call allocates for the evaluation.
 struct EvalPlan {
     jb_ctx* c;
+    Scratch scratch;
     int n_lo = 0;
     size_t L = 1, rows = 1, rpb = 1, count = 0;
     dim3 grid;
@@ -203,12 +205,7 @@ struct EvalPlan {
     unsigned long long* d_lanes = nullptr;   // the outputs' lanes, then one word for the bad-address flag
     size_t nlanes = 0;
     std::vector<EvalCol> cols;
-    explicit EvalPlan(jb_ctx* ctx) : c(ctx) {}
-    ~EvalPlan() {
-        c->dev_free(d_e);
-        c->dev_free(d_cols);
-        c->dev_free(d_lanes);
-    }
+    explicit EvalPlan(jb_ctx* ctx) : c(ctx), scratch(ctx) {}
     const uint64_t* e_hi() const { return d_e; }
     const uint64_t* e_lo() const { return d_e + 4 * rows; }
     unsigned int* bad() const { return reinterpret_cast<unsigned int*>(d_lanes + nlanes); }
@@ -220,9 +217,9 @@ struct EvalPlan {
         rows = (size_t)1 << (nvars - n_lo);
         count = cols.size();
         nlanes = count * lanes_per_output;
-        int st = c->dev_alloc((void**)&d_e, (rows + L) * 32);
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_cols, count * sizeof(EvalCol));
-        if (st == JB_OK) st = c->dev_alloc((void**)&d_lanes, (nlanes + 1) * 8);
+        int st = scratch.alloc((rows + L) * 32, &d_e);
+        if (st == JB_OK) st = scratch.alloc(count * sizeof(EvalCol), &d_cols);
+        if (st == JB_OK) st = scratch.alloc((nlanes + 1) * 8, &d_lanes);
         if (st != JB_OK) return st;
         st = c->check(cudaMemsetAsync(d_lanes, 0, (nlanes + 1) * 8, c->stream), "evaluate lanes memset");
         if (st == JB_OK)
@@ -354,7 +351,6 @@ int jb_small_evaluate_batch(jb_ctx* c, const void* const* columns, size_t count,
     if (count == 0) return JB_OK;
     Guard g(c);
     EvalPlan p(c);
-    Columns cols(c);
     // one launch per kind: the outputs are grouped by kind, each keeping its own lane block
     std::vector<size_t> first(SK_LAST + 2, 0);
     for (int k = SK_U8; k <= SK_LAST; ++k) {
@@ -362,7 +358,7 @@ int jb_small_evaluate_batch(jb_ctx* c, const void* const* columns, size_t count,
         for (size_t i = 0; i < count && st == JB_OK; ++i) {
             if (kinds[i] != k) continue;
             const void* d = nullptr;
-            st = cols.get(columns[i], len * (size_t)small_kind_bytes(k), on_device, &d);
+            st = get_column(p.scratch, columns[i], len * (size_t)small_kind_bytes(k), on_device, &d);
             p.cols.push_back(EvalCol{d, i});
         }
     }
@@ -389,14 +385,13 @@ int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int
     const uint64_t* r_addr = layout == JB_ONE_HOT_CYCLE_MAJOR ? point + 4 * log_t : point;
     Guard g(c);
     EvalPlan p(c);
-    Columns cols(c);
     for (size_t i = 0; i < count && st == JB_OK; ++i) {
         const void* d = nullptr;
-        st = cols.get(columns[i], T * (size_t)small_kind_bytes(kind), on_device, &d);
+        st = get_column(p.scratch, columns[i], T * (size_t)small_kind_bytes(kind), on_device, &d);
         p.cols.push_back(EvalCol{d, i});
     }
     uint64_t* d_eq = nullptr;
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_eq, K * 32);
+    if (st == JB_OK) st = p.scratch.alloc(K * 32, &d_eq);
     if (st == JB_OK) st = eq_build(c, r_addr, log_k, nullptr, d_eq);
     if (st == JB_OK) st = p.begin(r_cycle, log_t, 17);
     if (st == JB_OK) {
@@ -407,7 +402,6 @@ int jb_one_hot_evaluate(jb_ctx* c, const void* const* columns, size_t count, int
                      : launch_eval(p, OneHotSrc<SK_U16, false>{d_eq, (uint32_t)K, p.bad(), kind}, 0, count);
     }
     if (st == JB_OK) st = p.finish(out, nullptr);
-    c->dev_free(d_eq);
     return st;
 }
 
@@ -421,10 +415,10 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
     if ((st = check_point(c, r_cycle, log_t, "one_hot_pushforward: null point")) != JB_OK) return st;
     if (count == 0) return JB_OK;
     Guard g(c);
-    Columns cols(c);
+    Scratch scratch(c);
     std::vector<const void*> dcols(count, nullptr);
     for (size_t i = 0; i < count && st == JB_OK; ++i)
-        st = cols.get(columns[i], T * (size_t)small_kind_bytes(kind), on_device, &dcols[i]);
+        st = get_column(scratch, columns[i], T * (size_t)small_kind_bytes(kind), on_device, &dcols[i]);
     // the tables are handed out only once the bins are known to be valid
     std::vector<Table> made(count);
     std::vector<uint64_t*> bufs(count, nullptr);
@@ -435,15 +429,8 @@ int jb_one_hot_pushforward(jb_ctx* c, const void* const* columns, size_t count, 
     }
     if (st == JB_OK) st = one_hot_pushforward_into(c, dcols.data(), count, kind, T, K, r_cycle, bufs.data());
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "pushforward tables sync");
-    if (st != JB_OK) {
-        for (Table& t : made) c->release(t);
-        return st;
-    }
-    for (size_t i = 0; i < count; ++i) {
-        out_tables[i] = c->next_id++;
-        c->tables[out_tables[i]] = made[i];
-    }
-    return JB_OK;
+    for (size_t i = 0; i < count; ++i) c->hand_over(st, made[i], &out_tables[i]);
+    return st;
 }
 
 }  // extern "C"

@@ -935,23 +935,24 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
     uint64_t *buckets = nullptr, *partial = nullptr, *seg = nullptr, *win = nullptr, *d_out = nullptr;
     uint64_t *tree_a = nullptr, *tree_b = nullptr;
     const size_t tree_pts = (size_t)Weff * ((p.T + 2047) / 2048) + 1;
-    int st = c->dev_alloc((void**)&digits, (size_t)p.W * n * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&sorted, entries * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&hist, nb * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&offsets, (nb + 1) * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&toff, (nb + 1) * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&block_sums, 2 * 1024 * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&task_bucket, max_tasks * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&order, max_tasks * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&len_hist, 2 * MSM_LEN_BINS * 4);
+    Scratch scratch(c);
+    int st = scratch.alloc((size_t)p.W * n * 4, &digits);
+    if (st == JB_OK) st = scratch.alloc(entries * 4, &sorted);
+    if (st == JB_OK) st = scratch.alloc(nb * 4, &hist);
+    if (st == JB_OK) st = scratch.alloc((nb + 1) * 4, &offsets);
+    if (st == JB_OK) st = scratch.alloc((nb + 1) * 4, &toff);
+    if (st == JB_OK) st = scratch.alloc(2 * 1024 * 4, &block_sums);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 4, &task_bucket);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 4, &order);
+    if (st == JB_OK) st = scratch.alloc(2 * MSM_LEN_BINS * 4, &len_hist);
     if (st == JB_OK) st = c->check(cudaMemsetAsync(len_hist, 0, 2 * MSM_LEN_BINS * 4, c->stream), "msm memset");
-    if (st == JB_OK) st = c->dev_alloc((void**)&buckets, nb * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&partial, max_tasks * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&seg, (size_t)Weff * p.T * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&win, (size_t)Weff * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&tree_a, tree_pts * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&tree_b, tree_pts * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_out, 96 * rows);
+    if (st == JB_OK) st = scratch.alloc(nb * 128, &buckets);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 128, &partial);
+    if (st == JB_OK) st = scratch.alloc((size_t)Weff * p.T * 128, &seg);
+    if (st == JB_OK) st = scratch.alloc((size_t)Weff * 128, &win);
+    if (st == JB_OK) st = scratch.alloc(tree_pts * 128, &tree_a);
+    if (st == JB_OK) st = scratch.alloc(tree_pts * 128, &tree_b);
+    if (st == JB_OK) st = scratch.alloc(96 * rows, &d_out);
     if (st == JB_OK) st = c->check(cudaMemsetAsync(hist, 0, nb * 4, c->stream), "msm memset");
     if (st == JB_OK) {
         unsigned g = (unsigned)((n + 255) / 256);
@@ -1016,22 +1017,6 @@ int msm_device(jb_ctx* c, const Srs& srs, size_t offset, const void* d_scalars, 
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "msm sync");
         if (st == JB_OK) std::memcpy(out_xyz, c->h_small, 96);
     }
-    c->dev_free(digits);
-    c->dev_free(sorted);
-    c->dev_free(task_bucket);
-    c->dev_free(order);
-    c->dev_free(len_hist);
-    c->dev_free(hist);
-    c->dev_free(offsets);
-    c->dev_free(toff);
-    c->dev_free(block_sums);
-    c->dev_free(buckets);
-    c->dev_free(partial);
-    c->dev_free(seg);
-    c->dev_free(win);
-    c->dev_free(tree_a);
-    c->dev_free(tree_b);
-    c->dev_free(d_out);
     return st;
 }
 
@@ -1065,22 +1050,23 @@ int one_hot_device(jb_ctx* c, const Srs& srs, const void* const* columns, size_t
     uint32_t *sorted = nullptr, *task_bucket = nullptr, *order = nullptr;
     unsigned int *hist = nullptr, *offsets = nullptr, *toff = nullptr, *block_sums = nullptr, *len_hist = nullptr, *d_bad = nullptr;
     uint64_t *buckets = nullptr, *partial = nullptr, *d_out = nullptr;
-    int st = c->dev_alloc(&d_cols, count * T * esz);
+    Scratch scratch(c);
+    int st = scratch.alloc(count * T * esz, &d_cols);
     for (size_t p = 0; p < count && st == JB_OK; ++p)
         st = c->check(cudaMemcpyAsync((char*)d_cols + p * T * esz, columns[p], T * esz, cudaMemcpyHostToDevice, c->stream),
                       "one_hot_rows columns H2D");
-    if (st == JB_OK) st = c->dev_alloc((void**)&sorted, cap * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&hist, step * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&offsets, (step + 1) * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&toff, (step + 1) * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&block_sums, 2 * 1024 * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&task_bucket, max_tasks * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&order, max_tasks * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&len_hist, 2 * MSM_LEN_BINS * 4);
-    if (st == JB_OK) st = c->dev_alloc((void**)&buckets, step * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&partial, max_tasks * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_out, step * 96);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_bad, 4);
+    if (st == JB_OK) st = scratch.alloc(cap * 4, &sorted);
+    if (st == JB_OK) st = scratch.alloc(step * 4, &hist);
+    if (st == JB_OK) st = scratch.alloc((step + 1) * 4, &offsets);
+    if (st == JB_OK) st = scratch.alloc((step + 1) * 4, &toff);
+    if (st == JB_OK) st = scratch.alloc(2 * 1024 * 4, &block_sums);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 4, &task_bucket);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 4, &order);
+    if (st == JB_OK) st = scratch.alloc(2 * MSM_LEN_BINS * 4, &len_hist);
+    if (st == JB_OK) st = scratch.alloc(step * 128, &buckets);
+    if (st == JB_OK) st = scratch.alloc(max_tasks * 128, &partial);
+    if (st == JB_OK) st = scratch.alloc(step * 96, &d_out);
+    if (st == JB_OK) st = scratch.alloc(4, &d_bad);
     if (st == JB_OK) st = c->check(cudaMemsetAsync(d_bad, 0, 4, c->stream), "one_hot_rows memset");
     for (size_t b0 = 0; b0 < total && st == JB_OK; b0 += step) {
         const size_t nb = std::min(step, total - b0);
@@ -1108,19 +1094,6 @@ int one_hot_device(jb_ctx* c, const Srs& srs, const void* const* columns, size_t
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "one_hot_rows sync");
     if (st == JB_OK && *(const unsigned int*)c->h_small)
         st = fail_bad_address(c);
-    c->dev_free(d_cols);
-    c->dev_free(sorted);
-    c->dev_free(hist);
-    c->dev_free(offsets);
-    c->dev_free(toff);
-    c->dev_free(block_sums);
-    c->dev_free(task_bucket);
-    c->dev_free(order);
-    c->dev_free(len_hist);
-    c->dev_free(buckets);
-    c->dev_free(partial);
-    c->dev_free(d_out);
-    c->dev_free(d_bad);
     return st;
 }
 
@@ -1156,11 +1129,12 @@ void identity_xyz(uint64_t out[12]);
 int msm_binary_device(jb_ctx* c, const Srs& srs, size_t offset, const uint8_t* d_flags, size_t n, uint64_t out_xyz[12]) {
     const unsigned blocks = (unsigned)c->sm_count * 8;  // 8 blocks x 128 threads per SM (1056 on H100)
     const size_t T = (size_t)blocks * 128;
+    Scratch scratch(c);
     uint64_t *partial = nullptr, *tree_a = nullptr, *tree_b = nullptr, *d_out = nullptr;
-    int st = c->dev_alloc((void**)&partial, T * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&tree_a, ((T + 2047) / 2048 + 1) * 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&tree_b, 128);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_out, 96);
+    int st = scratch.alloc(T * 128, &partial);
+    if (st == JB_OK) st = scratch.alloc(((T + 2047) / 2048 + 1) * 128, &tree_a);
+    if (st == JB_OK) st = scratch.alloc(128, &tree_b);
+    if (st == JB_OK) st = scratch.alloc(96, &d_out);
     if (st == JB_OK) {
         int tix = c->timing_begin(4, n, 1);
         msm_select_sum_kernel<<<blocks, 128, 0, c->stream>>>(d_flags, srs.xy + 8 * offset, n, partial);
@@ -1175,10 +1149,6 @@ int msm_binary_device(jb_ctx* c, const Srs& srs, size_t offset, const uint8_t* d
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(c->h_small, d_out, 96, cudaMemcpyDeviceToHost, c->stream), "msm D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "msm sync");
     if (st == JB_OK) std::memcpy(out_xyz, c->h_small, 96);
-    c->dev_free(partial);
-    c->dev_free(tree_a);
-    c->dev_free(tree_b);
-    c->dev_free(d_out);
     return st;
 }
 
@@ -1191,6 +1161,19 @@ void identity_xyz(uint64_t out[12]) {
     std::memset(out + 8, 0, 32);
 }
 
+// The checks the single-MSM entry points share once their handles are found, in this order: terms [offset, offset + n)
+// within the bases and n <= scalars, no terms (out_xyz = the identity), fewer than 2^31 terms. The caller returns
+// unless the status is JB_OK and n > 0.
+int msm_checks(jb_ctx* c, const Srs& srs, size_t offset, size_t n, size_t scalars, uint64_t out_xyz[12]) {
+    if (n > scalars || offset + n > srs.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
+    if (n == 0) {
+        identity_xyz(out_xyz);
+        return JB_OK;
+    }
+    if (n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "msm: n must be < 2^31");
+    return JB_OK;
+}
+
 }  // namespace
 
 // HyperKZG open (hyperkzg.cu): the commitments of the h - 1 folded polynomials of lengths 2^(h-1) .. 2, packed back to
@@ -1200,9 +1183,9 @@ void identity_xyz(uint64_t out[12]) {
 int jb::msm_halving_rows_device(jb_ctx* c, jb_srs h_srs, const uint64_t* d_scalars, int h, uint64_t* out_xyz) {
     if (!c || !d_scalars || !out_xyz || h < 3 || h > 20) return JB_ERR_UNSUPPORTED;
     Guard g(c);
-    auto it = c->srs.find(h_srs);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    const Srs& srs = it->second;
+    Srs* found = nullptr;
+    if (const int st = c->find_srs(h_srs, &found)) return st;
+    const Srs& srs = *found;
     if (!srs.pre_small || srs.pre_small_len < ((size_t)1 << (h - 1))) return JB_ERR_UNSUPPORTED;
     return msm_device(c, srs, 0, d_scalars, ((size_t)1 << h) - 2, out_xyz, SK_FR, (size_t)(h - 1), h);
 }
@@ -1217,18 +1200,9 @@ int jb_srs_upload_affine(jb_ctx* c, const uint64_t* xy, size_t n, jb_srs* out) {
     Srs s;
     s.n = n;
     int st = c->dev_alloc((void**)&s.xy, (n ? n : 1) * 64);
-    if (st != JB_OK) return st;
-    if (n) {
-        st = c->check(cudaMemcpyAsync(s.xy, xy, n * 64, cudaMemcpyHostToDevice, c->stream), "srs H2D");
-        if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "srs H2D sync");
-        if (st != JB_OK) {
-            c->dev_free(s.xy);
-            return st;
-        }
-    }
-    *out = c->next_id++;
-    c->srs[*out] = s;
-    return JB_OK;
+    if (st == JB_OK && n) st = c->check(cudaMemcpyAsync(s.xy, xy, n * 64, cudaMemcpyHostToDevice, c->stream), "srs H2D");
+    if (st == JB_OK && n) st = c->check(cudaStreamSynchronize(c->stream), "srs H2D sync");
+    return c->hand_over(st, s, out);
 }
 
 int jb_srs_upload_jacobian(jb_ctx* c, const uint64_t* xyz, size_t n, jb_srs* out) {
@@ -1236,13 +1210,13 @@ int jb_srs_upload_jacobian(jb_ctx* c, const uint64_t* xyz, size_t n, jb_srs* out
     Guard g(c);
     for (size_t i = 0; i < n * 3; ++i)
         if (!canonical_q(xyz + 4 * i)) return c->fail(JB_ERR_INVALID, "srs: coordinate limbs not canonical (>= q)");
+    Scratch scratch(c);
     Srs s;
     s.n = n;
     uint64_t* d_xyz = nullptr;
     int st = c->dev_alloc((void**)&s.xy, (n ? n : 1) * 64);
-    if (st != JB_OK) return st;
-    if (n) {
-        st = c->dev_alloc((void**)&d_xyz, n * 96);
+    if (st == JB_OK && n) {
+        st = scratch.alloc(n * 96, &d_xyz);
         if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_xyz, xyz, n * 96, cudaMemcpyHostToDevice, c->stream), "srs H2D");
         if (st == JB_OK) {
             jacobian_to_affine_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(d_xyz, n, s.xy);
@@ -1250,26 +1224,20 @@ int jb_srs_upload_jacobian(jb_ctx* c, const uint64_t* xyz, size_t n, jb_srs* out
             st = c->check(cudaGetLastError(), "jacobian_to_affine launch");
         }
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "srs sync");
-        if (d_xyz) c->dev_free(d_xyz);
-        if (st != JB_OK) {
-            c->dev_free(s.xy);
-            return st;
-        }
     }
-    *out = c->next_id++;
-    c->srs[*out] = s;
-    return JB_OK;
+    return c->hand_over(st, s, out);
 }
 
 int jb_srs_generate_multiples(jb_ctx* c, const uint64_t base_xy[8], size_t n, jb_srs* out) {
     if (!c || !out || !base_xy || n == 0) return JB_ERR_INVALID;
     Guard g(c);
     if (!canonical_q(base_xy) || !canonical_q(base_xy + 4)) return c->fail(JB_ERR_INVALID, "srs: base limbs not canonical");
+    Scratch scratch(c);
     Srs s;
     s.n = n;
     uint64_t* d_base = nullptr;
     int st = c->dev_alloc((void**)&s.xy, n * 64);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_base, 64);
+    if (st == JB_OK) st = scratch.alloc(64, &d_base);
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_base, base_xy, 64, cudaMemcpyHostToDevice, c->stream), "srs base H2D");
     if (st == JB_OK) {
         size_t threads = (n + GEN_RUN - 1) / GEN_RUN;
@@ -1278,22 +1246,15 @@ int jb_srs_generate_multiples(jb_ctx* c, const uint64_t base_xy[8], size_t n, jb
         st = c->check(cudaGetLastError(), "gen_multiples launch");
     }
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "srs generate sync");
-    if (d_base) c->dev_free(d_base);
-    if (st != JB_OK) {
-        if (s.xy) c->dev_free(s.xy);
-        return st;
-    }
-    *out = c->next_id++;
-    c->srs[*out] = s;
-    return JB_OK;
+    return c->hand_over(st, s, out);
 }
 
 int jb_srs_precompute(jb_ctx* c, jb_srs h, int window_bits) {
     if (!c) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    Srs& s = it->second;
+    Srs* found = nullptr;
+    if (const int st = c->find_srs(h, &found)) return st;
+    Srs& s = *found;
     if (s.pre) return JB_OK;
     if (s.n == 0) return c->fail(JB_ERR_INVALID, "srs precompute: empty srs");
     const int cbits = window_bits > 0 ? window_bits : shared_window_for(s.n);
@@ -1320,19 +1281,19 @@ int jb_srs_precompute(jb_ctx* c, jb_srs h, int window_bits) {
 int jb_srs_len(jb_ctx* c, jb_srs h, size_t* n) {
     if (!c || !n) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    *n = it->second.n;
+    Srs* s = nullptr;
+    if (const int st = c->find_srs(h, &s)) return st;
+    *n = s->n;
     return JB_OK;
 }
 
 int jb_srs_download_affine(jb_ctx* c, jb_srs h, uint64_t* out_xy, size_t n) {
     if (!c || !out_xy) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (n > it->second.n) return c->fail(JB_ERR_INVALID, "srs download: n exceeds length");
-    int st = c->check(cudaMemcpyAsync(out_xy, it->second.xy, n * 64, cudaMemcpyDeviceToHost, c->stream), "srs D2H");
+    Srs* s = nullptr;
+    if (const int st = c->find_srs(h, &s)) return st;
+    if (n > s->n) return c->fail(JB_ERR_INVALID, "srs download: n exceeds length");
+    int st = c->check(cudaMemcpyAsync(out_xy, s->xy, n * 64, cudaMemcpyDeviceToHost, c->stream), "srs D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "srs D2H sync");
     return st;
 }
@@ -1340,32 +1301,25 @@ int jb_srs_download_affine(jb_ctx* c, jb_srs h, uint64_t* out_xy, size_t n) {
 int jb_srs_free(jb_ctx* c, jb_srs h) {
     if (!c) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    c->dev_free(it->second.xy);
-    if (it->second.pre) c->dev_free(it->second.pre);
-    if (it->second.pre_small) c->dev_free(it->second.pre_small);
-    c->srs.erase(it);
+    Srs* s = nullptr;
+    if (const int st = c->find_srs(h, &s)) return st;
+    c->release(*s);
+    c->srs.erase(h);
     return JB_OK;
 }
 
 int jb_msm_g1(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* scalars, size_t n, uint64_t out_xyz[12]) {
     if (!c || !out_xyz || (n && !scalars)) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (offset + n > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
-    if (n == 0) {
-        identity_xyz(out_xyz);
-        return JB_OK;
-    }
-    if (n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "msm: n must be < 2^31");
+    Srs* s = nullptr;
+    int st = c->find_srs(h, &s);
+    if (st == JB_OK) st = msm_checks(c, *s, offset, n, n, out_xyz);
+    if (st != JB_OK || n == 0) return st;
+    Scratch scratch(c);
     uint64_t* d_s = nullptr;
-    int st = c->dev_alloc((void**)&d_s, n * 32);
-    if (st != JB_OK) return st;
-    st = c->check(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, c->stream), "msm scalars H2D");
-    if (st == JB_OK) st = msm_device(c, it->second, offset, d_s, n, out_xyz);
-    c->dev_free(d_s);
+    st = scratch.alloc(n * 32, &d_s);
+    if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, c->stream), "msm scalars H2D");
+    if (st == JB_OK) st = msm_device(c, *s, offset, d_s, n, out_xyz);
     return st;
 }
 
@@ -1373,26 +1327,22 @@ int jb_msm_g1_small(jb_ctx* c, jb_srs h, size_t offset, const void* scalars, siz
     if (!c || !out_xyz || (n && !scalars)) return JB_ERR_INVALID;
     if (!compact_kind(kind)) return c->fail(JB_ERR_INVALID, "msm_small: unknown scalar kind");
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (offset + n > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
-    if (n == 0) {
-        identity_xyz(out_xyz);
-        return JB_OK;
-    }
-    if (n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "msm: n must be < 2^31");
+    Srs* s = nullptr;
+    int st = c->find_srs(h, &s);
+    if (st == JB_OK) st = msm_checks(c, *s, offset, n, n, out_xyz);
+    if (st != JB_OK || n == 0) return st;
+    Scratch scratch(c);
     void* d_s = nullptr;
     const size_t bytes = n * (size_t)small_kind_bytes(kind);
-    int st = c->dev_alloc(&d_s, bytes);
-    if (st != JB_OK) return st;
-    st = c->check(cudaMemcpyAsync(d_s, scalars, bytes, cudaMemcpyHostToDevice, c->stream), "msm small scalars H2D");
+    st = scratch.alloc(bytes, &d_s);
+    if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_s, scalars, bytes, cudaMemcpyHostToDevice, c->stream), "msm small scalars H2D");
     // The reference's dispatch for u8 / bool columns (msm/mod.rs:35-47, 96-106): all zero -> identity, all <= 1 ->
     // msm_binary, else msm_u8. One pass over the bytes decides (the reference's par_iter().all()); below 2^14 terms
     // the general path is launch-latency either way.
     unsigned int vmax = 2;
     if (st == JB_OK && kind == SK_U8 && n >= ((size_t)1 << 14)) {
         unsigned int* d_max = nullptr;
-        st = c->dev_alloc((void**)&d_max, 4);
+        st = scratch.alloc(4, &d_max);
         if (st == JB_OK) st = c->check(cudaMemsetAsync(d_max, 0, 4, c->stream), "msm max memset");
         if (st == JB_OK) {
             u8_max_kernel<<<(unsigned)c->sm_count * 4, 256, 0, c->stream>>>((const uint8_t*)d_s, n, d_max);
@@ -1401,14 +1351,12 @@ int jb_msm_g1_small(jb_ctx* c, jb_srs h, size_t offset, const void* scalars, siz
         }
         if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "msm max sync");
         if (st == JB_OK) std::memcpy(&vmax, c->h_small, 4);
-        if (d_max) c->dev_free(d_max);
     }
     if (st == JB_OK) {
         if (vmax == 0) identity_xyz(out_xyz);
-        else if (vmax == 1) st = msm_binary_device(c, it->second, offset, (const uint8_t*)d_s, n, out_xyz);
-        else st = msm_device(c, it->second, offset, d_s, n, out_xyz, kind);
+        else if (vmax == 1) st = msm_binary_device(c, *s, offset, (const uint8_t*)d_s, n, out_xyz);
+        else st = msm_device(c, *s, offset, d_s, n, out_xyz, kind);
     }
-    c->dev_free(d_s);
     return st;
 }
 
@@ -1418,9 +1366,9 @@ int jb_msm_g1_batch(jb_ctx* c, jb_srs h, size_t count, const void* const* scalar
     size_t srs_n = 0;
     {
         Guard g(c);
-        auto it = c->srs.find(h);
-        if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-        srs_n = it->second.n;
+        Srs* s = nullptr;
+        if (const int st = c->find_srs(h, &s)) return st;
+        srs_n = s->n;
         for (size_t k = 0; k < count; ++k) {
             if (kinds[k] != SK_FR && !compact_kind(kinds[k])) return c->fail(JB_ERR_INVALID, "batch_msm: unknown scalar kind");
             if (lens[k] > srs_n) return c->fail(JB_ERR_LENGTH, "batch_msm: a column is longer than the base set");
@@ -1448,10 +1396,11 @@ int jb_msm_g1_rows(jb_ctx* c, jb_srs h, const void* scalars, size_t rows, size_t
         return kind == SK_FR ? jb_msm_g1(c, h, 0, (const uint64_t*)scalars, row_width, out_xyz)
                              : jb_msm_g1_small(c, h, 0, scalars, row_width, kind, out_xyz);
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (row_width > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
-    int st = build_small_table(c, it->second, row_width);
+    Srs* s = nullptr;
+    int st = c->find_srs(h, &s);
+    if (st != JB_OK) return st;
+    if (row_width > s->n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
+    st = build_small_table(c, *s, row_width);
     if (st != JB_OK) return st;
     // rows per pass: 32-bit offsets (entries < 2^28 keeps the workspace near 2 GiB) and <= 4 Mi histogram counters
     const MsmPlan p = plan_with(8, small_kind_bits(kind));
@@ -1462,19 +1411,12 @@ int jb_msm_g1_rows(jb_ctx* c, jb_srs h, const void* scalars, size_t rows, size_t
     for (size_t r0 = 0; r0 < rows && st == JB_OK; r0 += per) {
         size_t cnt = rows - r0 < per ? rows - r0 : per;
         const char* src = (const char*)scalars + r0 * row_width * esz;
-        if (cnt == 1) {  // a lone last row: the single-MSM path (by_rows needs >= 2 rows)
-            void* d1 = nullptr;
-            st = c->dev_alloc(&d1, row_width * esz);
-            if (st == JB_OK) st = c->check(cudaMemcpyAsync(d1, src, row_width * esz, cudaMemcpyHostToDevice, c->stream), "msm rows H2D");
-            if (st == JB_OK) st = msm_device(c, it->second, 0, d1, row_width, out_xyz + 12 * r0, kind);
-            if (d1) c->dev_free(d1);
-            continue;
-        }
+        Scratch scratch(c);
         void* d_s = nullptr;
-        st = c->dev_alloc(&d_s, cnt * row_width * esz);
+        st = scratch.alloc(cnt * row_width * esz, &d_s);
         if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_s, src, cnt * row_width * esz, cudaMemcpyHostToDevice, c->stream), "msm rows H2D");
-        if (st == JB_OK) st = msm_device(c, it->second, 0, d_s, cnt * row_width, out_xyz + 12 * r0, kind, cnt);
-        if (d_s) c->dev_free(d_s);
+        // a lone last row takes the single-MSM path (by_rows needs >= 2 rows)
+        if (st == JB_OK) st = msm_device(c, *s, 0, d_s, cnt * row_width, out_xyz + 12 * r0, kind, cnt);
     }
     return st;
 }
@@ -1495,27 +1437,23 @@ int jb_msm_g1_one_hot_rows(jb_ctx* c, jb_srs h, const void* const* columns, size
         if (!columns[p]) return c->fail(JB_ERR_INVALID, "one_hot_rows: null column");
     const int log_w = log2_of(row_width), log_r = log_k + log_t - log_w;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (row_width > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
+    Srs* s = nullptr;
+    if (const int st = c->find_srs(h, &s)) return st;
+    if (row_width > s->n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
     if (log_r >= 32 || count >= ((size_t)1 << (32 - log_r)))
         return c->fail(JB_ERR_UNSUPPORTED, "one_hot_rows: count x R must be < 2^32");
-    return one_hot_device(c, it->second, columns, count, kind, log_t, log_k, log_w, layout == JB_ONE_HOT_ADDRESS_MAJOR ? 1 : 0,
+    return one_hot_device(c, *s, columns, count, kind, log_t, log_k, log_w, layout == JB_ONE_HOT_ADDRESS_MAJOR ? 1 : 0,
                           out_xyz);
 }
 
 int jb_msm_g1_device(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* d_scalars, size_t n, uint64_t out_xyz[12]) {
     if (!c || !out_xyz || (n && !d_scalars)) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
-    if (offset + n > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
-    if (n == 0) {
-        identity_xyz(out_xyz);
-        return JB_OK;
-    }
-    if (n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "msm: n must be < 2^31");
-    return msm_device(c, it->second, offset, d_scalars, n, out_xyz);
+    Srs* s = nullptr;
+    int st = c->find_srs(h, &s);
+    if (st == JB_OK) st = msm_checks(c, *s, offset, n, n, out_xyz);
+    if (st != JB_OK || n == 0) return st;
+    return msm_device(c, *s, offset, d_scalars, n, out_xyz);
 }
 
 // Multi-GPU MSM (SURVEY 8e): the terms are partitioned across ranks (each rank holds its own bases and
@@ -1528,10 +1466,11 @@ int jb_msm_g1_sharded(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* scalar
     int st = jb_msm_g1(c, h, offset, scalars, n, local);
     if (st != JB_OK) return st;
     Guard g(c);
+    Scratch scratch(c);
     uint64_t *d_mine = nullptr, *d_all = nullptr, *d_out = nullptr;
-    st = c->dev_alloc((void**)&d_mine, 96);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_all, 96 * (size_t)c->world);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_out, 96);
+    st = scratch.alloc(96, &d_mine);
+    if (st == JB_OK) st = scratch.alloc(96 * (size_t)c->world, &d_all);
+    if (st == JB_OK) st = scratch.alloc(96, &d_out);
     std::memcpy(c->h_small, local, 96);
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(d_mine, c->h_small, 96, cudaMemcpyHostToDevice, c->stream), "sharded msm H2D");
     if (st == JB_OK) st = c->comm_allgather(d_mine, d_all, 12);
@@ -1543,26 +1482,19 @@ int jb_msm_g1_sharded(jb_ctx* c, jb_srs h, size_t offset, const uint64_t* scalar
     if (st == JB_OK) st = c->check(cudaMemcpyAsync(c->h_small, d_out, 96, cudaMemcpyDeviceToHost, c->stream), "sharded msm D2H");
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "sharded msm sync");
     if (st == JB_OK) std::memcpy(out_xyz, c->h_small, 96);
-    c->dev_free(d_mine);
-    c->dev_free(d_all);
-    c->dev_free(d_out);
     return st;
 }
 
 int jb_msm_g1_table(jb_ctx* c, jb_srs h, size_t offset, jb_table scalars, size_t n, uint64_t out_xyz[12]) {
     if (!c || !out_xyz) return JB_ERR_INVALID;
     Guard g(c);
-    auto it = c->srs.find(h);
-    if (it == c->srs.end()) return c->fail(JB_ERR_INVALID, "unknown srs handle");
+    Srs* s = nullptr;
+    if (const int st = c->find_srs(h, &s)) return st;
     Table* t = c->find(scalars);
     if (!t) return c->fail(JB_ERR_INVALID, "unknown table handle");
-    if (n > t->len || offset + n > it->second.n) return c->fail(JB_ERR_LENGTH, "msm: bases/scalars length mismatch");
-    if (n == 0) {
-        identity_xyz(out_xyz);
-        return JB_OK;
-    }
-    if (n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "msm: n must be < 2^31");
-    return msm_device(c, it->second, offset, t->buf, n, out_xyz);
+    const int st = msm_checks(c, *s, offset, n, t->len, out_xyz);
+    if (st != JB_OK || n == 0) return st;
+    return msm_device(c, *s, offset, t->buf, n, out_xyz);
 }
 
 }  // extern "C"

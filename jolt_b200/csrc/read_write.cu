@@ -366,9 +366,9 @@ int load_field(jb_ctx* c, const jb_source& s, size_t n, uint64_t* out) {
     if (s.type == JB_SOURCE_TABLE)
         return c->check(cudaMemcpyAsync(out, c->find(s.table)->buf, n * 32, cudaMemcpyDeviceToDevice, c->stream),
                         "read-write: table copy");
-    Columns cols(c);
+    Scratch scratch(c);
     const void* d = nullptr;
-    int st = cols.get(s.values, n * (size_t)small_kind_bytes(s.kind), s.on_device, &d);
+    int st = get_column(scratch, s.values, n * (size_t)small_kind_bytes(s.kind), s.on_device, &d);
     if (st != JB_OK) return st;
     rw_load_kernel<<<grid_for(c, n), RW_BLOCK, 0, c->stream>>>(d, s.kind, n, out);
     return c->check(cudaGetLastError(), "rw_load_kernel launch");
@@ -500,12 +500,12 @@ int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_k
     }
     // the rows of the unbound matrix, straight from the borrowed columns
     unsigned* d_bad = nullptr;
-    Columns owned(c);
+    Scratch scratch(c);
     RwCols rc;
     std::memset(&rc, 0, sizeof rc);
     rc.addr_kind = addr_kind;
     rc.w = (int)w;
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_bad, sizeof(unsigned));
+    if (st == JB_OK) st = scratch.alloc(sizeof(unsigned), &d_bad);
     if (st == JB_OK) st = c->check(cudaMemsetAsync(d_bad, 0, sizeof(unsigned), c->stream), "read-write: flag memset");
     if (st == JB_OK) st = load_field(c, *inc, T, rw->inc.buf);
     if (st == JB_OK) st = load_field(c, *init, K, rw->init);
@@ -514,11 +514,11 @@ int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_k
         for (size_t b = 0; b < a && same == a; ++b)
             if (acc[b].addr == acc[a].addr) same = b;
         if (same < a) rc.addr[a] = rc.addr[same];
-        else st = owned.get(acc[a].addr, T * (size_t)small_kind_bytes(addr_kind), addr_on_device, &rc.addr[a]);
+        else st = get_column(scratch, acc[a].addr, T * (size_t)small_kind_bytes(addr_kind), addr_on_device, &rc.addr[a]);
         const jb_source& v = acc[a].value;
         rc.val_kind[a] = v.type == JB_SOURCE_TABLE ? SK_FR : v.kind;
         if (st == JB_OK && v.type == JB_SOURCE_TABLE) rc.val[a] = c->find(v.table)->buf;
-        else if (st == JB_OK) st = owned.get(v.values, T * (size_t)small_kind_bytes(v.kind), v.on_device, &rc.val[a]);
+        else if (st == JB_OK) st = get_column(scratch, v.values, T * (size_t)small_kind_bytes(v.kind), v.on_device, &rc.val[a]);
     }
     if (st == JB_OK) {
         by_a<CountL>((int)A, c, rc, *rw, d_bad);
@@ -542,7 +542,6 @@ int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_k
         st = c->check(cudaGetLastError(), "rw_fill_kernel launch");
     }
     if (st == JB_OK) st = read_count(c, *rw);  // (also: the borrowed columns have been read when this returns)
-    c->dev_free(d_bad);
     if (st != JB_OK) {  // (the caller holds the context lock: no jb_member_destroy here)
         rw_release(mem);
         for (auto& tb : mem->tables) c->release(tb);

@@ -147,10 +147,11 @@ int lt_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, 
         return c->check(cudaGetLastError(), "lt_expand_kernel launch");
     }
     const size_t hi_vars = nvars - EQ_BLOCK_VARS;
+    Scratch scratch(c);
     uint64_t *d_e = nullptr, *d_lt = nullptr, *d_lo = nullptr;
-    int st = c->dev_alloc((void**)&d_e, ((size_t)1 << hi_vars) * 32);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_lt, ((size_t)1 << hi_vars) * 32);
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_lo, (256 + 8) * 32);
+    int st = scratch.alloc(((size_t)1 << hi_vars) * 32, &d_e);
+    if (st == JB_OK) st = scratch.alloc(((size_t)1 << hi_vars) * 32, &d_lt);
+    if (st == JB_OK) st = scratch.alloc((256 + 8) * 32, &d_lo);
     if (st == JB_OK) st = eq_build(c, r, hi_vars, scale, d_e);
     if (st == JB_OK) st = lt_build(c, r, hi_vars, scale, d_lt);
     const uint64_t* r3 = r + 4 * hi_vars;
@@ -171,9 +172,6 @@ int lt_build(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t* scale, 
         c->launches++;
         st = c->check(cudaGetLastError(), "lt_stream_kernel launch");
     }
-    c->dev_free(d_e);
-    c->dev_free(d_lt);
-    c->dev_free(d_lo);
     return st;
 }
 
@@ -193,13 +191,7 @@ int structured_table(jb_ctx* c, const uint64_t* r, size_t nvars, const uint64_t*
     t.cap = t.len + extra;
     int st = c->dev_alloc((void**)&t.buf, t.cap * 32);
     if (st == JB_OK) st = fill(t.buf);
-    if (st != JB_OK) {
-        c->release(t);
-        return st;
-    }
-    *out = c->next_id++;
-    c->tables[*out] = t;
-    return JB_OK;
+    return c->hand_over(st, t, out);
 }
 
 }  // namespace

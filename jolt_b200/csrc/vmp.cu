@@ -216,8 +216,8 @@ int jb_lc_vector_matrix_product(jb_ctx* c, const jb_lc_term* terms, size_t count
     const Table* L = c->find(left);
     if (!L) return c->fail(JB_ERR_INVALID, "vector_matrix_product: unknown left table handle");
     if (L->len != R) return c->fail(JB_ERR_INVALID, "vector_matrix_product: the left table must have len / row_width entries");
-    Columns cols(c);
-    st = load_columns(cols, terms, count, desc);
+    Scratch scratch(c);
+    st = load_columns(scratch, terms, count, desc);
     std::vector<LcTerm> gather, scatter;
     size_t rows = 1;  // rows of the longest gather term
     for (const LcTerm& t : desc) {
@@ -230,8 +230,8 @@ int jb_lc_vector_matrix_product(jb_ctx* c, const jb_lc_term* terms, size_t count
     }
     LcTerm* d_terms = nullptr;
     unsigned long long* d_bins = nullptr;  // W bins of 8 lanes, then the bad-address flag
-    if (st == JB_OK && !gather.empty()) st = c->dev_alloc((void**)&d_terms, gather.size() * sizeof(LcTerm));
-    if (st == JB_OK) st = c->dev_alloc((void**)&d_bins, (W * 8 + 1) * 8);
+    if (st == JB_OK && !gather.empty()) st = scratch.alloc(gather.size() * sizeof(LcTerm), &d_terms);
+    if (st == JB_OK) st = scratch.alloc((W * 8 + 1) * 8, &d_bins);
     unsigned int* d_bad = reinterpret_cast<unsigned int*>(d_bins + W * 8);
     if (st == JB_OK) st = c->check(cudaMemsetAsync(d_bins, 0, (W * 8 + 1) * 8, c->stream), "vector_matrix_product bins");
     if (st == JB_OK && !gather.empty()) {
@@ -274,16 +274,8 @@ int jb_lc_vector_matrix_product(jb_ctx* c, const jb_lc_term* terms, size_t count
         st = launch_check(c, "bins_to_fr_kernel launch");
     }
     if (st == JB_OK) st = c->check(cudaStreamSynchronize(c->stream), "vector_matrix_product output sync");
-    c->dev_free(d_terms);
-    c->dev_free(d_bins);
-    if (st != JB_OK) {
-        c->dev_free(t.buf);
-        return st;
-    }
     t.cap = t.len = W;
-    *out = c->next_id++;
-    c->tables[*out] = t;
-    return JB_OK;
+    return c->hand_over(st, t, out);
 }
 
 }  // extern "C"
