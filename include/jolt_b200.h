@@ -314,7 +314,8 @@ int jb_member_create_product_sources(jb_ctx* ctx, const jb_source* sources, size
  *  - Precondition, relied on and not checked (checking needs a sort by address; a prover trusts its witness the same
  *    way): v_a(j) = Val(addr_a(j), j) wherever addr_a(j) is not none - the read values the witness holds.
  *  - w_cycle: nvars = t coordinates, w[0] <-> the most significant bit of j; optional scale. Variables are bound
- *    LowToHigh on x (the only order): first the t cycle bits, LSB first, then the kappa address bits.
+ *    LowToHigh on x (the only order): first the t cycle bits, LSB first, then the kappa address bits
+ *    (jb_member_create_read_write_phases puts the address bits after fewer cycle bits).
  *  - degree 3; t + kappa rounds; the running claim is mandatory in prove_round. The cycle rounds keep the eq factor
  *    split as jb_eq_member_create does and cost O(live entries) each: the matrix is kept as entries per (row, address)
  *    and a round pairs adjacent rows. After the t-th bind the one remaining row becomes K-entry field tables and the
@@ -341,6 +342,31 @@ int jb_member_create_read_write(jb_ctx* ctx, const jb_rw_access* accesses, size_
                                 int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
                                 const jb_source* init, const uint64_t* w_cycle, size_t nvars, const uint64_t* scale_or_null,
                                 int order, jb_member** out);
+/* Read-write checking member with the address rounds after p = cycle_rounds_first cycle rounds, 0 <= p <= t: the
+ * relation, its degree, round count, running claim and final values are jb_member_create_read_write's (which is
+ * this call with p = t, and runs exactly that code), but the rounds bind, LSB first,
+ *   rounds 0 .. p-1: cycle bits 0 .. p-1;   rounds p .. p+kappa-1: address bits 0 .. kappa-1;
+ *   rounds p+kappa .. t+kappa-1: cycle bits p .. t-1
+ * i.e. LowToHigh over x = (j >> p) K 2^p + k 2^p + (j mod 2^p). So r_cycle (MSB first) is the reverse of
+ * ch[0 .. p) ++ ch[p+kappa .. t+kappa) and r_addr the reverse of ch[p .. p+kappa); final_evals are ra_0 .. ra_{A-1},
+ * Val and inc at (r_addr, r_cycle) and jb_eq_member_scalar returns scale * eq(w_cycle, r_cycle). K = 1 has no address
+ * rounds: every p gives the rounds of p = t.
+ *  - The first p rounds are the sparse cycle rounds. Then the entries are sorted by (key, row) (a stable radix sort by
+ *    key) and the address rounds pair keys 2k', 2k'+1 in O(live entries) each: a key absent at a row takes ra = 0 and
+ *    Val = the ve of its own last entry at an earlier row, or its bound init value. Each row carries the weight
+ *    scale * eq(w_cycle over the bound cycle bits, their challenges) * eq(w[0 .. t-p), row). An address round has
+ *    degree 2 (s(3) is extrapolated). The remaining t - p cycle rounds run as an expression member over dense
+ *    T' = T / 2^p-entry tables ra_a, Val and the bound inc, with the eq factor split over w[0 .. t-p).
+ *  - Memory at creation, p < t and K > 1, besides the entry buffers of jb_member_create_read_write: the sort workspace
+ *    (shared with the scan's; about 8 bytes per entry of capacity), 2 x (K + 1) key offsets, the bound init table
+ *    (1.5 * 32 K bytes) and the dense tables ra_a, Val with their half-size bind buffers, 1.5 (A + 1) * 32 T' bytes
+ *    (inc is the bound inc table); the K-entry address tables are not allocated. JB_ERR_OOM can only arise here.
+ * Errors: those of jb_member_create_read_write, in its order, then JB_ERR_INVALID for cycle_rounds_first > t. */
+int jb_member_create_read_write_phases(jb_ctx* ctx, const jb_rw_access* accesses, size_t naccesses, size_t write_access,
+                                       int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
+                                       const jb_source* init, const uint64_t* w_cycle, size_t nvars,
+                                       const uint64_t* scale_or_null, size_t cycle_rounds_first, int order,
+                                       jb_member** out);
 /* Booleanity member (Shout's booleanity check on the RA polynomials): ProveRounds for
  *   sum_{k<K} sum_{j<T} scale * eq(r_addr, k) * eq(r_cycle, j) * sum_{i<d} c_i * (ra_i(k, j)^2 - ra_i(k, j)),
  *   ra_i(k, j) = [addr_i(j) = k]   (0 where addr_i(j) is the none value),

@@ -68,6 +68,10 @@ SIGNATURES = {
     "jb_member_create_read_write": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, ctypes.c_int, ctypes.c_int,
                                                    c_size_t, c_size_t, c_void_p, c_void_p, c_u64p, c_size_t, c_u64p,
                                                    ctypes.c_int, ctypes.POINTER(c_void_p)]),
+    "jb_member_create_read_write_phases": (ctypes.c_int, [c_void_p, c_void_p, c_size_t, c_size_t, ctypes.c_int,
+                                                          ctypes.c_int, c_size_t, c_size_t, c_void_p, c_void_p, c_u64p,
+                                                          c_size_t, c_u64p, c_size_t, ctypes.c_int,
+                                                          ctypes.POINTER(c_void_p)]),
     "jb_member_create_booleanity": (ctypes.c_int, [c_void_p, ctypes.POINTER(c_void_p), c_size_t, ctypes.c_int, ctypes.c_int,
                                                    c_size_t, c_size_t, c_u64p, c_u64p, c_u64p, c_u64p, ctypes.c_int,
                                                    ctypes.POINTER(c_void_p)]),

@@ -966,10 +966,13 @@ class ReadWriteCheckingMember(ExpressionMember):
     value = no access; accesses may share one column), the values v_a(j) = Val(addr_a(j), j) the witness holds (a Source.table or Source.compact, or anything
     Source.compact takes), c_a (an int or 4 Montgomery limbs) and d_a in {0, 1}; access `write` is the write. `inc`
     (T entries) and `init` (K entries) likewise. Everything is borrowed for the call. Degree 3, log2 T + log2 K rounds,
-    LowToHigh only; the running claim is mandatory. final_evals() returns ra_0 .. ra_{A-1}, Val, inc at the point."""
+    LowToHigh only; the running claim is mandatory. final_evals() returns ra_0 .. ra_{A-1}, Val, inc at the point.
+    cycle_rounds_first = p (None: log2 T) binds the first p cycle bits, then the log2 K address bits, then the
+    remaining cycle bits (jb_member_create_read_write_phases): r_cycle is then the reverse of the challenges of rounds
+    [0, p) and [p + log2 K, ...), r_addr the reverse of those of rounds [p, p + log2 K)."""
 
     def __init__(self, session: Session, accesses, write: int, inc, init, K: int, w_cycle, scale=None,
-                 order: int = LOW_TO_HIGH):
+                 order: int = LOW_TO_HIGH, cycle_rounds_first=None):
         def src(x):
             return x if isinstance(x, Source) else Source.compact(x)
         ptrs, kind, T, dev, keep = _address_columns([a[0] for a in accesses], "ReadWriteCheckingMember", u32=True)
@@ -987,10 +990,14 @@ class ReadWriteCheckingMember(ExpressionMember):
         if dev or any(isinstance(k, Source) and k.on_device for k in keep):
             session.after_torch()
         h = ctypes.c_void_p()
-        session.check(session.lib.jb_member_create_read_write(
-            session.h, ctypes.cast(arr, ctypes.c_void_p), len(accesses), write, kind, dev, T, K,
-            ctypes.cast(ctypes.pointer(inc_c), ctypes.c_void_p), ctypes.cast(ctypes.pointer(init_c), ctypes.c_void_p),
-            _p(w) if w.shape[0] else None, w.shape[0], _p(sc) if sc is not None else None, order, ctypes.byref(h)))
+        args = [session.h, ctypes.cast(arr, ctypes.c_void_p), len(accesses), write, kind, dev, T, K,
+                ctypes.cast(ctypes.pointer(inc_c), ctypes.c_void_p), ctypes.cast(ctypes.pointer(init_c), ctypes.c_void_p),
+                _p(w) if w.shape[0] else None, w.shape[0], _p(sc) if sc is not None else None]
+        if cycle_rounds_first is None:
+            session.check(session.lib.jb_member_create_read_write(*args, order, ctypes.byref(h)))
+        else:
+            session.check(session.lib.jb_member_create_read_write_phases(*args, int(cycle_rounds_first), order,
+                                                                         ctypes.byref(h)))
         self.s = session
         self.h = h
         self.ntables = len(accesses) + 2

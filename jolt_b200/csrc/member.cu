@@ -704,15 +704,42 @@ static void eq_absorb_coord(jb_member* mem, const uint64_t* w, const uint64_t* r
 static void eq_absorb_bind(jb_member* mem, size_t var, const uint64_t* r) { eq_absorb_coord(mem, mem->eq_w.data() + 4 * var, r); }
 
 static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
+static int rw_key_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
+static int rw_end_keys(jb_member* mem, const uint64_t r[4]);
 static int bool_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals);
 static int eq_round_tail(jb_member* mem, const HostFr& l0, const HostFr& l1, const uint64_t* claim, size_t round,
                          uint64_t* out_evals);
+
+// The split-eq weights of LowToHigh cycle round `round` (its variable w[n - 1 - round] is the pair index's lowest).
+static EqRound eq_weights_l2h(const jb_member* mem, size_t round) {
+    EqRound er;
+    const size_t cur = mem->eq_n - round;  // unbound variables including the current one (index cur - 1)
+    const size_t head = cur - 1;
+    const size_t out_bits = head < mem->eq_split ? head : mem->eq_split;
+    const size_t in_bits = head - out_bits;
+    er.e_out = mem->eq_tabs + 4 * (((size_t)1 << out_bits) - 1);
+    er.e_in = mem->eq_tabs + 4 * (mem->eq_in_base + ((size_t)1 << in_bits) - 1);
+    er.in_bits = (int)in_bits;
+    return er;
+}
 
 static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
     jb_ctx* c = mem->ctx;
     if (!claim) return c->fail(JB_ERR_INVALID, "eq member: the running claim is required (Gruen hint s(0)+s(1))");
     const size_t n = mem->eq_n;
-    if (mem->kind == MemberKind::ReadWrite && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
+    if (mem->kind == MemberKind::ReadWrite) {
+        const RwState& rw = *mem->rw;
+        if (rw.p == n && round >= n) return rw_address_round(mem, bind, round, claim, out_evals);
+        if (rw.p < n && round >= rw.p) {  // mixed order: the address rounds, then cycle round p onwards
+            if (round < rw.p + rw.kappa) return rw_key_round(mem, bind, round, claim, out_evals);
+            if (round == rw.p + rw.kappa && bind) {  // the last address variable: the dense tables take over
+                const int st = rw_end_keys(mem, bind);
+                if (st != JB_OK) return st;
+                bind = nullptr;
+            }
+            round -= rw.kappa;
+        }
+    }
     if (mem->kind == MemberKind::Booleanity) {  // the address rounds come first; the cycle rounds are its eq rounds
         const size_t ka = mem->bl->log_k;
         if (round < ka) return bool_address_round(mem, bind, round, claim, out_evals);
@@ -733,14 +760,8 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     EqRound er;
     size_t cur_var;
     if (l2h) {
-        const size_t cur = n - round;  // unbound variables including the current one (index cur - 1)
-        const size_t head = cur - 1;
-        const size_t out_bits = head < mem->eq_split ? head : mem->eq_split;
-        const size_t in_bits = head - out_bits;
-        er.e_out = mem->eq_tabs + 4 * (((size_t)1 << out_bits) - 1);
-        er.e_in = mem->eq_tabs + 4 * (mem->eq_in_base + ((size_t)1 << in_bits) - 1);
-        er.in_bits = (int)in_bits;
-        cur_var = cur - 1;
+        er = eq_weights_l2h(mem, round);
+        cur_var = n - round - 1;
     } else {
         // HighToLow (split_eq.rs:233-257): the current variable is w[round]; the remaining ones w[round + 1 .. n)
         // are the pair index MSB-first: the unbound suffix of in_point = w[1 .. 1 + s) on top of out_point =
@@ -759,7 +780,8 @@ static int eq_prove_round(jb_member* mem, const uint64_t* bind, size_t round, co
     const HostFr wc = HostFr::from_limbs(mem->eq_w.data() + 4 * cur_var);
     const HostFr l1 = scalar * wc, l0 = scalar - l1;
     if (l1.is_zero()) return c->fail(JB_ERR_INVALID, "eq member: current eq evaluation at one must be invertible");
-    int st = mem->kind == MemberKind::ReadWrite    ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
+    int st = mem->kind == MemberKind::ReadWrite && mem->rw->cycles
+                 ? rw_cycle_round(mem, bind, er, round_out(c, nullptr, 0, nullptr))
              : mem->kind == MemberKind::Booleanity ? bool_cycle_pass(mem, bind, er, round_out(c, nullptr, 0, nullptr))
                                                    : member_round(mem, bind, true, nullptr, &er);
     if (st != JB_OK) return st;
@@ -1129,15 +1151,11 @@ int jb_member_create_product_sources(jb_ctx* c, const jb_source* sources, size_t
 }
 
 // ---- read-write checking member -------------------------------------------------------------------------
-// Binds a cycle variable of a read-write member (its eq factor has absorbed r); after the last one the member's address
-// rounds are the expression pass over its K-entry tables ra_0 .. ra_{A-1}, Val, inc: sum_k e sum_a c_a ra_a(k) (Val(k) +
-// d_a inc) with e = scale * eq(w_cycle, r_cycle), as monomials c_a e ra_a Val and c_a e ra_a inc.
-static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
+// The expression pass that finishes a read-write member, over its tables ra_0 .. ra_{A-1}, Val, inc: the monomials
+// c_a e ra_a Val and c_a e ra_a inc (d_a = 1).
+static void rw_make_expr(jb_member* mem, const HostFr& e) {
     RwState& rw = *mem->rw;
     const int A = rw.A;
-    int st = rw_cycle_bind(mem, r);
-    if (st != JB_OK || rw.rows > 1) return st;
-    const HostFr e = HostFr::from_limbs(mem->eq_scalar);
     jb_monomial mo[2 * RW_MAX_ACCESSES];
     size_t nm = 0;
     for (int a = 0; a < A; ++a)
@@ -1151,11 +1169,27 @@ static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
         }
     make_expr(mem, mo, nm, (size_t)A + 2, 2);
     rw.cycles = false;
+}
+
+// Binds a cycle variable of a read-write member (its eq factor has absorbed r); after the last one the member's address
+// rounds are the expression pass over its K-entry tables ra_0 .. ra_{A-1}, Val, inc: sum_k e sum_a c_a ra_a(k) (Val(k) +
+// d_a inc) with e = scale * eq(w_cycle, r_cycle).
+static int rw_bind_cycle(jb_member* mem, const uint64_t r[4]) {
+    int st = rw_cycle_bind(mem, r);
+    if (st != JB_OK || mem->rw->rows > 1) return st;
+    rw_make_expr(mem, HostFr::from_limbs(mem->eq_scalar));
     return JB_OK;
 }
 
+// An address round has degree 2; s(3) is extrapolated so the member keeps reporting degree 3.
+static void rw_extrapolate_s3(uint64_t* out_evals) {
+    const RoundConsts& rc = round_consts(2);
+    HostFr s3 = HostFr::zero();
+    for (int t = 0; t <= 2; ++t) s3 = s3 + rc.next[t] * HostFr::from_limbs(out_evals + 4 * t);
+    s3.store(out_evals + 12);
+}
+
 // An address round: the first one binds the last cycle variable and hands the member over to its expression pass.
-// The round polynomial has degree 2; s(3) is extrapolated so the member keeps reporting degree 3.
 static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
     jb_ctx* c = mem->ctx;
     if (round == mem->eq_n) {
@@ -1166,27 +1200,71 @@ static int rw_address_round(jb_member* mem, const uint64_t* bind, size_t round, 
     }
     const int st = launched_round(mem, bind, !c->verify_rounds, claim, round, out_evals);  // s(0..2)
     if (st != JB_OK) return st;
-    const RoundConsts& rc = round_consts(2);
-    HostFr s3 = HostFr::zero();
-    for (int t = 0; t <= 2; ++t) s3 = s3 + rc.next[t] * HostFr::from_limbs(out_evals + 4 * t);
-    s3.store(out_evals + 12);
+    rw_extrapolate_s3(out_evals);
     return JB_OK;
+}
+
+// An address round of a mixed order (p < t cycle rounds first). The first one binds the p-th cycle variable (p > 0) and
+// re-sorts the entries by key; the others bind the previous address variable. The pass weights each row by
+// eq(w[0 .. t - p), row), the host multiplies the eq scalar in; s(1) comes from the claim unless rounds are verified.
+static int rw_key_round(jb_member* mem, const uint64_t* bind, size_t round, const uint64_t* claim, uint64_t* out_evals) {
+    jb_ctx* c = mem->ctx;
+    const RwState& rw = *mem->rw;
+    const size_t n = mem->eq_n;
+    int st = JB_OK;
+    if (round == rw.p && bind) {
+        eq_absorb_bind(mem, n - round, bind);
+        st = rw_cycle_bind(mem, bind);
+    }
+    if (st == JB_OK) st = round == rw.p ? rw_begin_keys(mem) : rw_key_bind(mem, bind);
+    if (st == JB_OK)
+        st = rw_key_pass(mem, eq_weights_l2h(mem, rw.p), mem->eq_w.data() + 4 * (n - rw.p - 1), round_out(c, nullptr, 0, nullptr));
+    if (st == JB_OK) st = wait_round_result0(c);
+    if (st != JB_OK) return st;
+    const bool skip1 = !c->verify_rounds;
+    const HostFr e = HostFr::from_limbs(mem->eq_scalar);
+    uint64_t vals[3 * 4];  // q(0), [q(1)], q(inf), scaled
+    int k = 0;
+    for (int i = 0; i < 3; ++i)
+        if (i != 1 || !skip1) (e * HostFr::from_limbs(c->h_result + 4 * i)).store(vals + 4 * k++);
+    if ((st = assemble_evals(c, 2, skip1, vals, claim, round, out_evals)) != JB_OK) return st;
+    rw_extrapolate_s3(out_evals);
+    return JB_OK;
+}
+
+// The last address bind of a mixed order: the remaining cycle rounds are the expression pass over the dense tables,
+// split-eq weighted over w[0 .. t - p) with the member's eq scalar.
+static int rw_end_keys(jb_member* mem, const uint64_t r[4]) {
+    const int st = rw_key_bind(mem, r);
+    if (st == JB_OK) rw_make_expr(mem, HostFr::one());
+    return st;
+}
+
+int jb_member_create_read_write_phases(jb_ctx* c, const jb_rw_access* accesses, size_t naccesses, size_t write_access,
+                                       int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
+                                       const jb_source* init, const uint64_t* w_cycle, size_t nvars,
+                                       const uint64_t* scale_or_null, size_t cycle_rounds_first, int order,
+                                       jb_member** out) {
+    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
+    jb_member* mem = nullptr;
+    {
+        Guard g(c);
+        const int st = rw_create(c, accesses, naccesses, write_access, addr_kind, addr_on_device, T, K, inc, init, w_cycle,
+                                 nvars, scale_or_null, cycle_rounds_first, order, &mem);
+        if (st != JB_OK) return st;
+    }
+    *out = mem;
+    return eq_setup(mem, w_cycle, nvars, scale_or_null, out);
 }
 
 int jb_member_create_read_write(jb_ctx* c, const jb_rw_access* accesses, size_t naccesses, size_t write_access,
                                 int addr_kind, int addr_on_device, size_t T, size_t K, const jb_source* inc,
                                 const jb_source* init, const uint64_t* w_cycle, size_t nvars, const uint64_t* scale_or_null,
                                 int order, jb_member** out) {
-    if (!c) return jb_device_count() > 0 ? JB_ERR_INVALID : JB_ERR_NO_DEVICE;  // without a device there is no context
-    jb_member* mem = nullptr;
-    {
-        Guard g(c);
-        const int st = rw_create(c, accesses, naccesses, write_access, addr_kind, addr_on_device, T, K, inc, init, w_cycle,
-                                 nvars, scale_or_null, order, &mem);
-        if (st != JB_OK) return st;
-    }
-    *out = mem;
-    return eq_setup(mem, w_cycle, nvars, scale_or_null, out);
+    // every cycle round first (p = log2 T; T itself is checked by rw_create)
+    const size_t t = T >= 1 && (T & (T - 1)) == 0 ? (size_t)log2_of(T) : 0;
+    return jb_member_create_read_write_phases(c, accesses, naccesses, write_access, addr_kind, addr_on_device, T, K, inc,
+                                              init, w_cycle, nvars, scale_or_null, t, order, out);
 }
 
 // ---- booleanity member ----------------------------------------------------------------------------------
@@ -1529,7 +1607,8 @@ int jb_member_finish_rounds(jb_member* mem, const uint64_t bind[4]) {
         if (st == JB_OK) mem->len = 1;
         return st;
     }
-    if (mem->eq && mem->kind != MemberKind::ReadWrite) {  // (a read-write member's address rounds have no eq factor)
+    // (the address rounds of a read-write member that binds every cycle variable first have no eq factor)
+    if (mem->eq && (mem->kind != MemberKind::ReadWrite || mem->rw->p < mem->eq_n)) {
         size_t var = 0;
         for (size_t l = mem->len; l > 2; l >>= 1) ++var;  // unbound variables besides the one being bound
         // LowToHigh binds w[var] (the most significant unbound one is w[0]); HighToLow binds w[n - 1 - var]

@@ -102,7 +102,7 @@ enum class MemberKind {
     Dense,       // a product or sum of products over field tables (also an expression that is exactly such a shape)
     Expr,        // the expression pass over tables or sources (ex)
     Product,     // the product of m <= 16 tables or sources (terms = 1) through product_round_kernel
-    ReadWrite,   // read-write checking (rw): sparse cycle rounds, then the expression pass over K-entry tables
+    ReadWrite,   // read-write checking (rw): sparse rounds, then the expression pass over the remaining tables
     Booleanity,  // booleanity (bl): address rounds, then cycle rounds
 };
 
@@ -161,7 +161,9 @@ struct jb_member {
     // bind writes the len/2 field entries. Cleared (and the columns released) by the bind.
     std::vector<SourceCol> src;
     // ReadWrite (jb_member_create_read_write): the sparse cycle phase until the last cycle variable is bound, then the
-    // expression pass over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (RwState::cycles)
+    // expression pass over the A + 2 K-entry tables ra_0 .. ra_{A-1}, Val, inc (RwState::cycles); with p < t cycle
+    // rounds first: p sparse cycle rounds, the sparse address rounds, then the eq-weighted expression pass over the
+    // A + 2 tables over the remaining rows
     struct RwState* rw = nullptr;
     // Booleanity (jb_member_create_booleanity): its d tables live in bl, not in `tables`
     struct BoolState* bl = nullptr;
@@ -180,39 +182,52 @@ struct EqWeights {
 
 // read_write.cu ----------------------------------------------------------------------------------------------
 constexpr int RW_MAX_ACCESSES = JB_RW_MAX_ACCESSES;
-// The cycle phase of a read-write checking member: the bound K x T matrix as entries sorted by (row, key), in two
-// buffers that take turns as the input and the output of a bind. Per entry and buffer: key and row (u32), the field
-// arrays ra_0 .. ra_{A-1}, val, vs (Val before the row's block of cycles) and ve (Val after it).
+// The sparse phases of a read-write checking member: the bound K x T matrix as entries in two buffers that take turns
+// as the input and the output of a bind. Per entry and buffer: key and row (u32), the field arrays ra_0 .. ra_{A-1},
+// val, vs (Val before the row's block of cycles) and ve (Val after it). The cycle phase keeps the entries sorted by
+// (row, key) and pairs rows; with p < t cycle rounds first the address phase then re-sorts them by (key, row) and pairs
+// keys (by_key; vs is unused).
 struct RwState {
-    bool cycles = true;  // the cycle phase; cleared when the last cycle variable is bound and ex is the address phase's
+    bool cycles = true;  // the sparse phases; cleared when the member's tables hold the expression pass's tables
+    bool by_key = false; // the address phase of a mixed order (p < t)
     int A = 0, w = 0;
     uint64_t coeff[RW_MAX_ACCESSES][4];
     int d[RW_MAX_ACCESSES];
     size_t T = 0, K = 0;
-    size_t rows = 0;  // rows of the bound matrix (T >> cycle variables bound)
+    size_t p = 0;      // cycle rounds before the address rounds (t: every cycle round first)
+    size_t kappa = 0;  // log2 K
+    size_t rows = 0;  // groups of the bound matrix: rows (T >> cycle variables bound), or keys in the address phase
     size_t n = 0;     // live entries
     size_t cap = 0;   // entries a buffer holds: min(K, distinct address columns) * T, which no bind exceeds
     int cur = 0;      // the buffer holding the current matrix
     uint32_t* key[2] = {nullptr, nullptr};
     uint32_t* row[2] = {nullptr, nullptr};
     uint64_t* f[2] = {nullptr, nullptr};    // (A + 3) x cap field elements
-    uint32_t* off[2] = {nullptr, nullptr};  // row offsets, rows + 1
-    uint32_t* flag = nullptr;               // cap + 1: the scan input
-    uint32_t* base = nullptr;               // cap + 1: the scan output
-    void* scan_tmp = nullptr;
+    uint32_t* off[2] = {nullptr, nullptr};  // group offsets, groups + 1
+    uint32_t* flag = nullptr;               // cap + 1: the scan input (the sort's input permutation)
+    uint32_t* base = nullptr;               // cap + 1: the scan output (the sort's output permutation)
+    void* scan_tmp = nullptr;               // the scan's and the sort's workspace
     size_t scan_bytes = 0;
-    Table inc;                 // inc(j) over the rows, bound alongside
-    uint64_t* init = nullptr;  // K initial values
+    Table inc;   // inc(j) over the rows, bound alongside
+    Table init;  // the K initial values, bound by the address rounds of a mixed order
 };
 // Checks and builds a read-write member without its eq factor (eq_setup adds it); nothing stays allocated on failure.
 int rw_create(jb_ctx* c, const jb_rw_access* acc, size_t A, size_t w, int addr_kind, int addr_on_device, size_t T,
               size_t K, const jb_source* inc, const jb_source* init, const uint64_t* w_cycle, size_t nvars,
-              const uint64_t* scale, int order, jb_member** out);
+              const uint64_t* scale, size_t cycle_rounds_first, int order, jb_member** out);
 // One cycle round: binds `bind` (if given), then the pass that leaves q(0), q(inf) in result slot ro.
 int rw_cycle_round(jb_member* mem, const uint64_t* bind, const EqWeights& eqw, jb::RoundOut ro);
 // Binds one cycle variable; after the last one the remaining row is scattered into the member's K-entry tables and
 // the cycle-phase buffers are released.
 int rw_cycle_bind(jb_member* mem, const uint64_t r[4]);
+// Mixed order, after the p-th cycle bind: the entries re-sorted by (key, row) with their key offsets.
+int rw_begin_keys(jb_member* mem);
+// An address round's pass: leaves the unscaled q(0), q(1), q(inf) in result slot ro; eqw and w_low (the lowest row
+// variable's coordinate) give the row weights eq(w[0 .. t - p), row).
+int rw_key_pass(jb_member* mem, const EqWeights& eqw, const uint64_t* w_low, jb::RoundOut ro);
+// Binds one address variable; after the last one the remaining key becomes the dense tables ra_a, Val, inc over the
+// T / 2^p rows and the sparse buffers are released.
+int rw_key_bind(jb_member* mem, const uint64_t r[4]);
 void rw_release(jb_member* mem);
 
 // booleanity.cu ----------------------------------------------------------------------------------------------

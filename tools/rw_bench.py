@@ -16,9 +16,13 @@ precondition and the rounds' cost does not depend on it, so the values are rando
 Dense route (registers, T = 2^20): the expression member over the materialised tables (ra_a, Val, inc and a replicated
 eq table, 6 x 2^27 entries) proving the same rounds, tables already on the device: dense_rounds_ms (every round + final
 evaluations, median of 2 after 1 warm-up) next to the member's rw_ms on the same columns; both agree round by round.
+With --cycle-rounds-first P,... every workload runs once per p (jb_member_create_read_write_phases; "t" and "t/2" stand
+for log2 T and its half) instead of the dense route, and also reports phase_ms: the host wall time of the p cycle
+rounds, of the log2 K address rounds and of the remaining cycle rounds (the first address round includes the re-sort by
+key, the first remaining cycle round the dense tables).
 Reads the card's name, power limit, maximum and current SM clock in the same run. One JSON line per workload on stdout, and in FILE with --out.
 
-usage: python tools/rw_bench.py [--out FILE] [--quick] [--only PREFIX]"""
+usage: python tools/rw_bench.py [--out FILE] [--quick] [--only PREFIX] [--cycle-rounds-first P,...]"""
 import argparse
 import json
 import pathlib
@@ -80,7 +84,7 @@ def live_entries(cols, K, T):
     return out
 
 
-def run(sess, wl, reps):
+def run(sess, wl, reps, p=None):
     K, T, cols, acc_spec, write = wl["K"], wl["T"], wl["cols"], wl["acc"], wl["write"]
     rng = np.random.default_rng(1)
     dev_cols = [torch.from_numpy(c.view({1: np.uint8, 2: np.int16, 4: np.int32}[c.itemsize])).cuda() for c in cols]
@@ -101,7 +105,8 @@ def run(sess, wl, reps):
     def once():
         t0 = time.perf_counter()
         acc = [(dev_cols[ci], Source.compact(vals[a], "u64"), coeffs[a], d) for a, (ci, d) in enumerate(acc_spec)]
-        m = ReadWriteCheckingMember(sess, acc, write, Source.compact(inc_t, "i64"), Source.compact(init_t, "u64"), K, w)
+        m = ReadWriteCheckingMember(sess, acc, write, Source.compact(inc_t, "i64"), Source.compact(init_t, "u64"), K, w,
+                                    cycle_rounds_first=p)
         times["create_ms"] = (time.perf_counter() - t0) * 1e3
         claim, bind, rounds = 1, None, []
         for rnd in range(t + kappa):
@@ -175,7 +180,13 @@ def main():
     ap.add_argument("--out")
     ap.add_argument("--quick", action="store_true", help="T = 2^16 only (a rehearsal)")
     ap.add_argument("--only", default=None, help="only the workloads whose name starts with this (no dense route)")
+    ap.add_argument("--cycle-rounds-first", default=None,
+                    help="comma-separated p values (integers, t or t/2): each workload once per p (no dense route)")
     args = ap.parse_args()
+    splits = args.cycle_rounds_first.split(",") if args.cycle_rounds_first else [None]
+
+    def resolve(tok, t):
+        return None if tok is None else t if tok == "t" else t // 2 if tok == "t/2" else int(tok)
     rng = np.random.default_rng(0)
     name, power = card()
     sess = jolt_b200.Session(0)
@@ -202,15 +213,22 @@ def main():
         live = live_entries(wl["cols"], wl["K"], wl["T"])
         ebytes = 8 + 32 * (A + 3)
         bound_bytes = sum((2 * live[m] + live[m + 1]) * ebytes for m in range(len(live) - 1))
-        ms, times = run(sess, wl, 3)
-        sm_max, sm_now = sm_clocks()
-        rec = dict(workload=wl["name"], K=wl["K"], T=wl["T"], A=A, ms=round(ms, 3), live=live,
-                   bound_ms=round(bound_bytes / HBM_BYTES_PER_S * 1e3, 3), entry_bytes=ebytes,
-                   create_ms=round(times["create_ms"], 3), round_ms=times["round_ms"], card=name, power_limit=power,
-                   sm_clock_max=sm_max, sm_clock_after=sm_now)
-        print(json.dumps(rec), flush=True)
-        lines.append(json.dumps(rec))
-    if not args.quick and not args.only:
+        t, kappa = wl["T"].bit_length() - 1, wl["K"].bit_length() - 1
+        for tok in splits:
+            p = resolve(tok, t)
+            ms, times = run(sess, wl, 3, p)
+            sm_max, sm_now = sm_clocks()
+            rec = dict(workload=wl["name"], K=wl["K"], T=wl["T"], A=A, ms=round(ms, 3), live=live,
+                       bound_ms=round(bound_bytes / HBM_BYTES_PER_S * 1e3, 3), entry_bytes=ebytes,
+                       create_ms=round(times["create_ms"], 3), round_ms=times["round_ms"], card=name, power_limit=power,
+                       sm_clock_max=sm_max, sm_clock_after=sm_now)
+            if p is not None:
+                r = times["round_ms"]
+                rec.update(cycle_rounds_first=p, phase_ms=[round(sum(r[:p]), 3), round(sum(r[p:p + kappa]), 3),
+                                                           round(sum(r[p + kappa:]), 3)])
+            print(json.dumps(rec), flush=True)
+            lines.append(json.dumps(rec))
+    if not args.quick and not args.only and splits == [None]:
         rec = dense_comparison(sess, 2)
         rec.update(card=name, power_limit=power, sm_clock_max=sm_clocks()[0])
         print(json.dumps(rec), flush=True)
