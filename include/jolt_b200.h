@@ -513,10 +513,11 @@ int jb_srs_upload_jacobian(jb_ctx* ctx, const uint64_t* xyz_limbs, size_t n, jb_
  * distinct curve points with a closed form for checking: msm(s) == (sum_i s_i (i+1)) * base. */
 int jb_srs_generate_multiples(jb_ctx* ctx, const uint64_t base_xy[8], size_t n, jb_srs* out);
 /* Optional, for a fixed SRS (HyperKZGProverSetup lives as long as the prover): builds the table
- * 2^(c w) * bases[i] for every window w (c = window_bits, 0 = choose from the SRS length), W x the SRS in
- * HBM (e.g. 12 x 1 GiB at 2^24). MSMs over this handle with n >= 2^(c-4) then use ONE bucket set for
+ * 2^(c w) * bases[i] for every window w (c = window_bits in 8..23, 0 = choose from the SRS length), W x the
+ * SRS in HBM (e.g. 12 x 1 GiB at 2^24). MSMs over this handle with n >= 2^(c-4) then use ONE bucket set for
  * all windows: wider windows (fewer bucket additions), no per-window reduction, no 2^(c w) doubling
- * chains. Results are identical group values. JB_ERR_OOM leaves the handle usable on the plain path. */
+ * chains. Results are identical group values. Other window bits are JB_ERR_INVALID (the bucket scan holds
+ * 2^(c-1) <= 4 Mi buckets). JB_ERR_INVALID and JB_ERR_OOM leave the handle usable on the plain path. */
 int jb_srs_precompute(jb_ctx* ctx, jb_srs s, int window_bits);
 int jb_srs_len(jb_ctx* ctx, jb_srs s, size_t* n);
 int jb_srs_download_affine(jb_ctx* ctx, jb_srs s, uint64_t* out_xy, size_t n);

@@ -1336,7 +1336,8 @@ class G1Bases:
 
     def precompute(self, window_bits: int = 0) -> "G1Bases":
         """Builds the 2^(c w) * P_i table for a fixed SRS (jb_srs_precompute): later large MSMs over this
-        handle share one bucket set across windows. Same group values."""
+        handle share one bucket set across windows. Same group values. `window_bits`: 8..23, or 0 to choose from
+        the SRS length; any other width raises JB_ERR_INVALID and leaves the handle on the plain per-window path."""
         self.s.check(self.s.lib.jb_srs_precompute(self.s.h, self.handle, window_bits))
         return self
 

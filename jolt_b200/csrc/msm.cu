@@ -864,6 +864,8 @@ using Guard = CtxGuard;
 
 // 2. the exclusive scans of the histogram `hist` (nb counters): bucket offsets, task offsets, and the histogram zeroed
 // into the scatter cursor. block_sums: 2 x 1024 counters (nb <= 4 Mi).
+// Every caller keeps nb <= 4 Mi (1024 scan blocks of 4096): msm_scan_blocks_kernel scans the block totals in ONE block of
+// 1024 threads, so a larger histogram would write past block_sums and leave the upper block bases unscanned.
 void launch_bucket_scan(jb_ctx* c, unsigned int* hist, unsigned int* offsets, unsigned int* toff, size_t nb,
                         unsigned int* block_sums, unsigned maxq) {
     const unsigned scan_blocks = (unsigned)((nb + SCAN_PER_BLOCK - 1) / SCAN_PER_BLOCK);
@@ -1258,7 +1260,8 @@ int jb_srs_precompute(jb_ctx* c, jb_srs h, int window_bits) {
     if (s.pre) return JB_OK;
     if (s.n == 0) return c->fail(JB_ERR_INVALID, "srs precompute: empty srs");
     const int cbits = window_bits > 0 ? window_bits : shared_window_for(s.n);
-    if (cbits < 8 || cbits > 24) return c->fail(JB_ERR_INVALID, "srs precompute: window bits must be in 8..24");
+    // c <= 23: the one bucket set of 2^(c-1) counters must fit the bucket scan (launch_bucket_scan, <= 4 Mi)
+    if (cbits < 8 || cbits > 23) return c->fail(JB_ERR_INVALID, "srs precompute: window bits must be in 8..23");
     const MsmPlan p = plan_with(cbits);
     if ((size_t)p.W * s.n >= ((size_t)1 << 31)) return c->fail(JB_ERR_UNSUPPORTED, "srs precompute: windows * bases must be < 2^31");
     int st = c->dev_alloc((void**)&s.pre, (size_t)p.W * s.n * 64);
